@@ -1,6 +1,6 @@
-# Top-level build: libsalmon_b200.so (CUDA, sm_100a only) + the oracle (test infra).
+# Top-level build: libsalmon_b200.so (CUDA, sm_90a only) + the oracle (test infra).
 NVCC      ?= /usr/local/cuda/bin/nvcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVCCFLAGS := -O3 -std=c++17 -lineinfo $(ARCH) -Xcompiler -fPIC -Xcompiler -Wall -Xcompiler -fopenmp $(PTXAS_V)
 CSRC      := salmon_b200/csrc
 LIB       := salmon_b200/libsalmon_b200.so

@@ -11,8 +11,10 @@ A "step" = one CollapsedEMOptimizer::optimize-equivalent run of 1000 iterations.
   e2e   : the same through sb_em_optimize with HOST buffers (pinned): H2D of the CSR
           table + device-side preparation (combined weights, both layouts) + 1000
           iterations + D2H of alpha, all inside the timed region.
-L2 is flushed (512 MB memset) before every timed step; inside a step the working set
-(~75 MB) is L2-resident by nature of the workload (the same table is swept 1000x).
+L2 is flushed (memset of twice the L2, at least 256 MB) before every timed step; inside a step the
+same ~75 MB table is swept 1000x.  It does not fit H100's 50 MB L2, and by default no part of it
+is pinned there (l2_keep_cm = l2_keep_tm = 0): the stream comes from HBM on every iteration; the
+gathered vectors (theta, scale: ~6 MB) fit in L2.
 
 N > 1 (torchrun, one rank per GPU): weak scaling -- every rank holds its OWN 500k-class
 table (the eq-classes of its read shard) and alpha is all-reduced once per iteration.
@@ -20,6 +22,11 @@ value = N x (iterations / s): 500k-class-shard iterations per second.
 
 --impl reference : the CPU path (oracle port, OpenMP over all host cores) on the same
 workload; each step is a bounded sample of iterations.
+
+--dump-outputs DIR : after the timed steps, what the timed paths returned in their last step
+(alpha of the resident run and of sb_em_optimize, the class table and per-transcript vectors of
+Stage A's finish()) as DIR/<name>.npy in float64, so that two builds can be compared output for
+output; the inputs are seeded and identical from run to run.
 """
 import argparse
 import json
@@ -27,6 +34,7 @@ import os
 import statistics
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -96,7 +104,7 @@ def measured_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (NVIDIA H100 SXM data sheet, 3.35 TB/s; not a measurement)"
 
 
 def algorithmic_bytes_per_iter(eq, vbem=True):
@@ -170,8 +178,34 @@ class ClockSampler:
                 "samples": len(sm), "window": window}
 
 
+def gpu_identity(index):
+    """name and power limit of the card the numbers are measured on (part of every number)"""
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30)
+        return r.stdout.strip() or None
+    except Exception:  # noqa: BLE001
+        return None
+
+
+def dump_outputs(d, arrays, budget):
+    """arrays: name -> array, written as float64 in at most `budget` bytes; an array larger than its share is replaced by
+    a fixed, seeded sample of its elements (their indices in <name>.index.npy).  EM and Stage A get 16 + 48 MB."""
+    os.makedirs(d, exist_ok=True)
+    share = budget // max(1, len(arrays)) // 8 // 2       # elements per array (values + sample indices)
+    for name, a in arrays.items():
+        a = np.asarray(a).ravel()
+        if a.size > share:
+            idx = np.sort(np.random.default_rng(12345).choice(a.size, share, replace=False))
+            np.save(os.path.join(d, name + ".index.npy"), idx.astype(np.float64))
+            a = a[idx]
+        np.save(os.path.join(d, name + ".npy"), a.astype(np.float64))
+
+
 _CPU_BEST = {}
-CPU_PROBE_FILE = os.path.join(ROOT, ".cpu_probe.json")     # git-ignored; per box (it does not travel back)
+# per machine and user: the thread-count probe is cached outside the tree (the tree may be read-only), named by uid so
+# that a file another user left in the shared temporary directory is never read
+CPU_PROBE_FILE = os.path.join(tempfile.gettempdir(), f"sb_bench_cpu_probe_{os.getuid()}.json")
 CPU_REPEATS = 5
 
 
@@ -191,7 +225,7 @@ def cpu_port_rate(eq, proj, eff, uniq, vbem, budget_s, threads):
     The port mirrors the reference's decomposition (parallel_for over classes + CAS f64 adds).  On many-core
     hosts that decomposition is contention-bound, so the thread count is chosen ONCE per box by a probe over
     {all, 64, 32, 16, 8} cores and the serial restatement (median of three differences per candidate); the
-    choice is written to .cpu_probe.json and reused by every later call on that box (the driver runs the
+    choice is written to CPU_PROBE_FILE and reused by every later call on that box (the driver runs the
     reference arm and then this arm on the same box: both time the same thread count).  Threads are pinned
     (OMP_PROC_BIND=close, OMP_PLACES=cores, set before libgomp loads).  The reported rate is the MEDIAN of
     CPU_REPEATS timed runs; returns (rate, iterations per run, threads, [rates])."""
@@ -251,15 +285,6 @@ def stage_a_algorithmic_bytes(n_frags, read_len, c, band=15):
     """SURVEY.md section 8d: B_frag = 2*len/4 + L*96 + E/4 + P*8 + A*(len+2*band)/4 + 32*K (+ 4*sum|label|)."""
     return (n_frags * 2 * read_len / 4 + c["lookups"] * 96 + c["postings"] * 8 + c["candidates"] * (read_len + 2 * band) / 4
             + 32 * c["kept"] + 4 * c["label_entries"])
-
-
-def stage_a_traffic(frags_per_launch):
-    """DRAM bytes per seed-kernel launch from the committed ncu --set full capture (per fragment x fragments per launch)"""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "traffic_r2.json")))["stage_a"]
-        return t["dram_bytes_per_fragment"] * frags_per_launch
-    except Exception:  # noqa: BLE001
-        return None
 
 
 def stage_a_workload(rank, small=False):
@@ -537,7 +562,6 @@ def bench_stage_a(args, rank, world, local, dist, W, peak, peak_src, ncores):
                      "frac": seed_achieved / peak, "peak_source": peak_src, "avg_launch_ms": seed_launch_ms,
                      "fragments_per_launch": frags_per_launch,
                      "algorithmic_bytes_per_launch": seed_bytes,
-                     "traffic": stage_a_traffic(frags_per_launch),
                      "whole_stage_algorithmic_gbs": stage_a_algorithmic_bytes(n, L, c) / res_t / 1e9,
                      "note": "the kernel is latency/issue-bound (dependent hash-probe -> posting loads, warp-level sort "
                              "and scans), not bandwidth-bound: see DESIGN.md"},
@@ -555,6 +579,10 @@ def bench_stage_a(args, rank, world, local, dist, W, peak, peak_src, ncores):
             out["from_files"] = stage_a_from_files(idx, left, right, batch, ncores)
     if ctx is not None:
         ctx.close()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"stage_a_" + k: res[k] for k in
+                                         ("off", "tids", "weights", "counts", "projected_counts", "eff_len", "unique_counts",
+                                          "total_counts")}, 48 << 20)
     return out
 
 
@@ -570,6 +598,7 @@ def main():
     ap.add_argument("--no-stage-a", action="store_true", help="skip the Stage A (mapping) measurement")
     ap.add_argument("--sa-small", action="store_true", help="Stage A on a 20x smaller transcriptome (dev)")
     ap.add_argument("--no-files", action="store_true", help="skip the FASTQ-files -> classes measurement (row f1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -610,7 +639,7 @@ def main():
             "cpu_baseline": {"value": val, "unit": "iters/s", "cores": used, "kind": "port", "host_cores": ncores,
                              "sample": f"median over steps; each step = median of {CPU_REPEATS} runs of {sample_iters} "
                                        f"iterations of the same workload; thread count probed once per box "
-                                       f"(best of all/64/32/16/8/serial, cached in .cpu_probe.json), threads pinned"},
+                                       f"(best of all/64/32/16/8/serial, cached per box), threads pinned"},
             "e2e": {"value": val, "unit": "iters/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
             "gpu_launches": 0,
         }
@@ -626,7 +655,7 @@ def main():
         print(json.dumps(line))
         return 0
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     from salmon_b200 import EMContext, default_params, _capi
     dist = None
     if world > 1:
@@ -687,7 +716,7 @@ def main():
     assert abs(alpha_sum - tot_counts) / tot_counts < 1e-9, (alpha_sum, tot_counts)
 
     # ---- end to end: sb_em_optimize, host buffers in/out
-    e2e_ms = []
+    e2e_ms, a2 = [], None
     for i in range(2 + args.steps):
         ctx.flush_l2()
         barrier()
@@ -732,6 +761,8 @@ def main():
                   "workload": f"the seed=1 table ({C2['C']} classes) round-robin split over {world} ranks"}
 
     peak, peak_src = measured_peak()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"em_alpha": alpha, "em_e2e_alpha": a2}, 16 << 20)
     ctx.close()
     stage_a = None
     if not args.no_stage_a:
@@ -746,10 +777,6 @@ def main():
     kern_iters_per_launch = ITERS_PER_STEP if fused else 1
     avg_launch_ms = loop_step_ms if fused else loop_step_ms / ITERS_PER_STEP
     achieved = b_iter * kern_iters_per_launch / (avg_launch_ms / 1e3) / 1e9
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "traffic_r2.json")
-    if os.path.exists(tp):
-        traffic = json.load(open(tp)).get("dram_bytes_per_launch")
     cpu_val, cpu_n, cpu_used, cpu_rates = (cpu_port_rate(eq, proj, eff, uniq, vbem, args.cpu_budget, ncores)
                                            if world == 1 else (None, 0, 0, []))
     line = {
@@ -759,7 +786,7 @@ def main():
         "config": config,
         "details": {"per_gpu_nnz": eq.nnz, "affinity_cores": len(_AFFINITY or []),
                    "l2": "flushed (memset > 2x L2) before every timed step; inside a step the table is re-swept "
-                         "1000x and stays L2-resident, as in production",
+                         "1000x; it exceeds L2 and nothing is pinned (l2_keep 0 / 0): it streams from HBM; the gathered theta / scale (~6 MB) fit in L2",
                    "parallelism": "1 GPU" if world == 1 else
                    f"classes sharded over {world} GPUs (own table per rank), alpha all-reduced per iteration "
                    f"({'ncclAllReduce' if args.nccl else 'inside the persistent kernel over NVLink peer memory'}); "
@@ -769,23 +796,24 @@ def main():
                     "k_em_persistent_mgpu: 1 cooperative launch per step per rank; partial alpha' pushed to owner slices as "
                     "flagged 16-byte lines over NVLink peer memory, theta' pushed back, no exchange barrier"),
                    "wall_s_resident_loop": wall_resident, "strong_scaling": strong},
-        "clocks": clocks,
+        "gpu": gpu_identity(local), "clocks": clocks,
         "e2e": {"value": e2e_value, "unit": "iters/s", "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),
                 "ms_per_step": e2e_step_ms, "api": "sb_em_optimize (C ABI, pinned host buffers)"},
         "gpu_launches": int(launches),
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": traffic, "peak_source": peak_src,
+                     "peak_source": peak_src,
                      "algorithmic_bytes_per_iteration": b_iter,
                      "kernel": "k_em_persistent" if world == 1 else
                      ("k_em_p1+k_em_p2_partial+k_em_update" if args.nccl else "k_em_persistent_mgpu"),
                      "avg_launch_ms": avg_launch_ms, "iterations_per_launch": kern_iters_per_launch,
-                     "note": "data is L2-resident by design, so DRAM traffic is far below the algorithmic bytes"},
+                     "note": "algorithmic bytes over kernel time (the gathered theta / scale fit in L2), "
+                             "not measured DRAM traffic"},
     }
     if cpu_val is not None:
         line["cpu_baseline"] = {"value": cpu_val, "unit": "iters/s", "cores": cpu_used, "kind": "port",
                                 "host_cores": ncores,
                                 "sample": f"median of {CPU_REPEATS} runs of {cpu_n} iterations of the same workload; thread "
-                                          f"count probed once per box (cached in .cpu_probe.json, shared with the "
+                                          f"count probed once per box (cached per box, shared with the "
                                           f"reference arm), threads pinned",
                                 "runs": [round(x, 1) for x in cpu_rates]}
     if stage_a is not None:

@@ -1,5 +1,5 @@
 /*
- * salmon_b200.h -- C ABI of libsalmon_b200.so (B200 / sm_100a).
+ * salmon_b200.h -- C ABI of libsalmon_b200.so (H100 / sm_90a).
  *
  * Drop-in boundary for Salmon's quantification hot path (SURVEY.md section 8b).
  * The reference has no FFI layer; the seams are ordinary C++ calls.  Each entry

@@ -1,7 +1,8 @@
 #!/usr/bin/env bash
 # oracle/build_ref.sh -- compile the reference's OWN translation units that build
-# standalone (no cmake, no external libraries) from where they lie under /root/reference,
-# outputs only into oracle/_ref/ (git-ignored, shipped to the GPU box by gpurun).
+# standalone (no cmake, no external libraries) from where they lie in a salmon source
+# tree ($REF), outputs only into oracle/_ref/ (git-ignored).  tests/golden/make_ref_golden.py
+# records what they return as the golden vectors the tests compare against.
 #
 #   src/xxhash.c   XXH64 used by TranscriptGroup::hash (src/model/TranscriptGroup.cpp:10-15)
 #   src/edlib.cpp  Myers edit distance used by recoverOrphans (--recoverOrphans)
@@ -11,7 +12,7 @@
 # Everything else on the path needs Boost / oneTBB / pufferfish (absent): unbuildable here,
 # see DESIGN.md section 2.  Reference SOURCES are never copied into the repo.
 set -euo pipefail
-REF=${REF:-/root/reference}
+REF=${REF:?"set REF to a salmon source tree"}
 HERE="$(cd "$(dirname "$0")" && pwd)"
 OUT="$HERE/_ref"
 mkdir -p "$OUT"

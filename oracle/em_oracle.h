@@ -15,7 +15,7 @@
  *     high-precision mpmath values (tests/golden/digamma_golden.json).
  *   - EMUpdate_/truncateCountVector (serial): pinned against the reference's
  *     own src/inference/EMUtils.cpp compiled into oracle/_ref (see
- *     oracle/build_ref.sh) when /root/reference is present.
+ *     oracle/build_ref.sh) from a salmon source tree.
  *   - the reference ships no golden vectors / KATs for this path
  *     (SURVEY.md section 4), so the remaining functions are pinned only by
  *     hand-derived tiny cases in tests/golden/.

@@ -6,7 +6,7 @@
  *
  * PARITY UNPINNED for the mapping core: rows a2-a4 live in COMBINE-lab/pufferfish @ ace68c1c
  * (MemCollector / MemChainer / joinReadsAndFilter / PuffAligner / ksw2pp), which is NOT in
- * /root/reference and has no tests or golden vectors in the salmon tree (SURVEY.md 8c).  The
+ * the salmon source tree and has no tests or golden vectors in the salmon tree (SURVEY.md 8c).  The
  * seed -> chain -> join -> banded-affine-DP algorithm below is this project's own, documented
  * in DESIGN.md ("Stage A, MAPSPEC"); it follows the call sites and option semantics salmon
  * shows (initMapperSettings, include/salmon/internal/quant/SalmonMappingUtils.hpp:153-223;

@@ -1,6 +1,6 @@
 // oracle/ref_shims/kseq_parse.cpp -- TEST INFRASTRUCTURE.  Glue around the FASTA/FASTQ parser the reference tree
 // vendors (include/kseq++.hpp, klibpp::KStream -- the parser behind salmon's read files): every record's sequence line,
-// as that parser delivers it.  Compiled by oracle/build_ref.sh against the header where it lies under /root/reference.
+// as that parser delivers it.  Compiled by oracle/build_ref.sh against the header where it lies in a salmon source tree.
 #include <zlib.h>
 
 #include <kseq++.hpp>

@@ -1,4 +1,4 @@
-"""salmon_b200 -- B200-native hot path of Salmon quantification.
+"""salmon_b200 -- H100-native (sm_90a) hot path of Salmon quantification.
 
 Only what the path needs: csrc/ (CUDA kernels + the C ABI in include/salmon_b200.h),
 the ctypes binding (_capi), the host-side mirror of the reference's optimiser

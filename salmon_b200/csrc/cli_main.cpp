@@ -71,7 +71,7 @@ struct Args {
 
 int usage() {
   fprintf(stderr,
-          "sb_salmon (salmon-b200 %d): B200-native hot path of salmon\n"
+          "sb_salmon (salmon-b200 %d): H100-native hot path of salmon\n"
           "  sb_salmon index -t transcripts.fa[.gz] -i index_dir [-k 31] [--gencode] [-d decoys.txt] [--keepDuplicates] [--no-clip]\n"
           "  sb_salmon quant -i index_dir -l IU|ISF|ISR -1 r1.fq[.gz] ... -2 r2.fq[.gz] ... | -l U|SF|SR -r reads.fq[.gz] ...  -o out_dir [--gpus N]\n"
           "                  [-p threads] [--dumpEq] [--dumpEqWeights]\n"

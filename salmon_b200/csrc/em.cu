@@ -1,4 +1,4 @@
-// em.cu -- Stage B: EM / VBEM over equivalence classes on B200 (sm_100a).
+// em.cu -- Stage B: EM / VBEM over equivalence classes on H100 (sm_90a).
 //
 // Replaces CollapsedEMOptimizer::optimize (src/inference/CollapsedEMOptimizer.cpp:732-1035)
 // and its update kernels EMUpdate_ (:178-234) / VBEMUpdate_ (:241-328).
@@ -66,8 +66,6 @@ static KernelSet make_set(const char* name) {
 }
 // chunk columns x ring depth x resident blocks per SM (shared memory per block = 8 warps x CH x RING x 384 B):
 //   0: 16x2 b2 (96 KB, 16 warps/SM)   1: 8x4 b2   2: 8x3 b3 (72 KB, 24 warps/SM)   3: 8x2 b4 (48 KB, 32 warps/SM)
-// Measured in round 2 and removed again (DESIGN.md section 3.4): a ring-less kernel with block-level dynamic
-// distribution, and gathers through a shared-memory window of theta / scale.
 constexpr int N_KERNEL_SETS = 4;
 static const KernelSet& kernel_set(int cfg) {
   static const KernelSet sets[N_KERNEL_SETS] = {
@@ -1027,7 +1025,7 @@ static void fill_args(sb_em_ctx* c, EmArgs& A, bool row_space) {
   A.cm.keep_pct = (uint32_t)c->keep_cm;
   A.tm.keep_pct = (uint32_t)c->keep_tm;
   // the bootstrap driver's overrides apply only while it is running (ov_active): the buffers outlive it, and a later
-  // optimize on the same context must not see the last replicate's resampled counts (ADVICE r1)
+  // optimize on the same context must not see the last replicate's resampled counts (bootstrap overrides)
   const bool ov = c->ov_active;
   A.c_cnt = (ov && c->ov_cnt) ? c->ov_cnt : c->d_cnt; A.scale = c->d_scale;
   if (row_space) {
@@ -1459,8 +1457,8 @@ extern "C" int sb_em_run(sb_em_ctx* c, sb_em_stats* stats) {
   return SB_OK;
 }
 
-// Measured re-balancing (VERDICT r1: 42 % of all warp time was spent waiting at the two grid barriers because the
-// static split by column count does not predict a warp's phase time).  One short instrumented run of the persistent
+// Measured re-balancing (a static split by column count does not predict a warp's phase time, and every warp waits
+// at the two grid barriers for the slowest).  One short instrumented run of the persistent
 // kernel accumulates, per warp, the duration of P1 and P2 and of their SELL parts (em_kernels.cuh: SB_ACC_*); the
 // slice ranges are then re-cut so that   long-row time of the warp (fixed: those rows are dealt by list position)
 // + sum over its slices of (measured time density of the warp that ran the slice x modelled slice cost)

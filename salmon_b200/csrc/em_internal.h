@@ -36,7 +36,7 @@ struct sb_em_ctx {
   // options
   int variant = 1;        // 1 = persistent cooperative kernel, 0 = one launch per phase
   int blocks_per_sm = 0;  // 0 = as many as fit
-  int config = 0;         // kernel configuration (ring chunk x depth x resident blocks), see kernel_set()
+  int config = 1;         // kernel configuration (ring chunk x depth x resident blocks), see kernel_set(); 8x4 b2 is the fastest on H100
   int rebalance = 1;      // rounds of measured re-cutting of the warp ranges at prepare (0 = column-count model only)
   int rebalance_iters = 8;
   int occ = 0;
@@ -45,7 +45,9 @@ struct sb_em_ctx {
   int sell_group_cm = 1024, sell_group_tm = 1024;   // rows per length-bucketing group (locality window of the gathers)
   int lwarp = 2048;                 // longest row reduced by one warp (longer: one block)
   int balance_long = 0;             // charge the long rows of a warp / block to its share of the slice stream
-  int keep_cm = 100, keep_tm = 30;  // % of stream chunks pinned in L2 (evict_last)  // per-slice epilogue cost (in columns) for the work split
+  // % of stream chunks pinned in L2 (evict_last).  0 on H100: the ~75 MB of the two layouts at configs[1] size are
+  // well beyond its 50 MB L2, and pinning any share of them measured slower (DESIGN.md section 3.4)
+  int keep_cm = 0, keep_tm = 0;
 
   // problem
   uint64_t C = 0, nnz = 0;

@@ -1,4 +1,4 @@
-// em_kernels.cuh -- the EM / VBEM iteration kernels (sm_100a).
+// em_kernels.cuh -- the EM / VBEM iteration kernels (sm_90a).
 //
 // One iteration = two segmented reductions over the class<->transcript map held
 // twice in HBM (class-major and transcript-major), no atomics on the data path,
@@ -18,13 +18,12 @@
 // count model, then re-cut from MEASURED per-warp phase times (em.cu: rebalance).
 // Rows longer than LMAX are reduced by a warp / a whole block from their CSR copy.
 //
-// Round 2 (VERDICT r1: 42 % of warp time at the grid barriers, the rest split between L2 gather
-// latency and dependent FP64 chains):
+// Design points (a warp's time goes to waiting at the grid barriers, L2 gather latency and dependent FP64 chains):
 //   * the consumption loop is software-pipelined over BATCHES of <= NB columns: the gathers of
 //     batch b+1 (and the epilogue operands of its slice) are issued before batch b is consumed
 //     and before the epilogue of a finished slice runs, so a slice costs max(gather round trip,
-//     epilogue chain) instead of their sum, and a short slice is ONE round trip (round 1: a
-//     4-wide batch plus one serialised round trip per remaining column);
+//     epilogue chain) instead of their sum, and a short slice is ONE round trip (not a 4-wide batch
+//     plus one serialised round trip per remaining column);
 //   * the VBEM epilogue is one branch-light function (em_math.h) instead of a Boost-style
 //     digamma with data-dependent loops followed by exp();
 //   * VBEM / EM are template parameters: the NaN guard of plain EM (:206) is compiled out of VBEM;
@@ -308,8 +307,8 @@ __device__ __forceinline__ void ring_drain(WarpCtx<CH, RING>& W, const WarpRange
 // entries have weight 0 and gather a slot that always holds 0.0): inside a group the layout is lane-major,
 //   idx[(group * 32 + lane) * 4 + j],  w[(group * 32 + lane) * 4 + j]        j = 0..3,
 // so a lane reads its four indices with ONE 16-byte shared-memory load and its four weights with two, issues the
-// four gathers together and needs no predicate and no remainder loop (round 1 / the first round-2 attempt spent
-// 10-12 instructions per column here; this is ~4).  Two groups (8 gathers) are in flight when a slice has them.
+// four gathers together and needs no predicate and no remainder loop (a per-column loop with predicated loads needs
+// several times the instructions per column).  Two groups (8 gathers) are in flight when a slice has them.
 template <int PHASE, int CH, int RING, bool VBEM, bool DYNQ, class Deliver>
 __device__ __forceinline__ void run_phase(const EmArgs& A, WarpCtx<CH, RING>& W, const WarpRange& R,
                                           uint32_t bid, uint32_t nblk, double logNorm, double bias,
@@ -429,8 +428,8 @@ __device__ __forceinline__ void run_phase(const EmArgs& A, WarpCtx<CH, RING>& W,
   // long rows (LMAX < len <= LWARP): one warp per row, lanes stride the CSR copy with four independent gathers in
   // flight, fixed shuffle tree.  Sorted longest-first.  Persistent kernels (DYNQ): taken one at a time from a global
   // queue by whichever warp has finished its SELL share (the next claim is in flight while a row is reduced), so the
-  // tail of a phase is filled evenly -- round 1 dealt them round-robin and the warp that drew a 1900-entry row ended
-  // the phase 6-12 us after the median.  Per-phase launches: dealt round-robin over the warps of the grid.
+  // tail of a phase is filled evenly -- dealt round-robin, the warp that draws the longest row ends the phase well
+  // after the others.  Per-phase launches: dealt round-robin over the warps of the grid.
   {
     const uint32_t gw = bid * EM_WARPS + (threadIdx.x >> 5);
     const uint32_t nw = nblk * EM_WARPS;
@@ -628,8 +627,8 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent(const __grid
 //     its {sum(alpha'+prior), max rel diff} into every rank's llaux
 //   unpack: every rank polls the llth lines of the other slices into its plain theta; block 0 polls the G x grid aux
 //     pairs and reduces them in (rank, block) order -> identical logNorm / convergence decision everywhere  -> grid barrier
-// Round 1 pulled the partials with remote loads between two exchange barriers (system fence + grid barrier + flag
-// round trip + grid barrier, every thread fencing at system scope): +41 us per iteration at N=2, +94 us at N=8.
+// Pushing flagged lines replaces pulling the partials with remote loads between two exchange barriers (system fence +
+// grid barrier + flag round trip + grid barrier, every thread fencing at system scope), which costs per iteration.
 __device__ __forceinline__ void st_release_sys(unsigned long long* p, unsigned long long v) {
   asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
@@ -758,10 +757,10 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent_mgpu(const _
       grid.sync();
       if (bid == 0 && threadIdx.x == 0) A.lq[1] = 0u;
       // ... and from there to the owners in transcript order: consecutive threads write consecutive 16-byte lines,
-      // i.e. whole 512-byte runs per warp over NVLink.  Measured (scripts/timeline_mgpu.py): at N=8 the pushes from
-      // the row epilogues below -- 32 scattered remote stores per warp instruction -- cost +10 us of P2, this pass
-      // is 6 us faster per iteration; at N=2 it is the other way round (one destination: 65 vs 45 us), so the host
-      // picks the pass for more than two ranks.
+      // i.e. whole 512-byte runs per warp over NVLink, instead of the row epilogues' pushes below (32 scattered
+      // remote stores per warp instruction).  With one destination (N=2) the epilogue pushes overlap P2 and the extra
+      // pass does not pay, so the host picks the pass for more than two ranks (scripts/timeline_mgpu.py times both;
+      // not measured on H100).
       for (uint32_t t = gtid; t < M; t += gthreads) push(t, __ldcg(&A.part_out[t]));
     } else {
       // straight from the row epilogues; locally inactive transcripts (constant share) first

@@ -2,8 +2,8 @@
 // (reference call sites: src/inference/CollapsedEMOptimizer.cpp:119-131,256-272: expTheta[i] =
 // exp(digamma(alpha_i + prior_i) - logNorm), 0 when alpha_i + prior_i <= digammaMin).
 //
-// Round 1 called a Boost-style digamma (log + divisions, a `while (x > 2) result += 1/x` recurrence) followed by
-// exp(): lanes of a warp took different paths, so a warp executed their union (~290 instructions per row, ncu r1).
+// A Boost-style digamma (log + divisions, a `while (x > 2) result += 1/x` recurrence) followed by exp() lets the
+// lanes of a warp take different paths, so a warp executes their union.
 // Here:  x' = x (x >= 10)  or  x + 10 (x < 10), and
 //     digamma(x) = ln x' - 1/(2x') - sum_{k=1..8} B_2k / (2k x'^2k) - [ 1/x + sum_{k=1..9} 1/(x+k) ]        (x < 10)
 // (recurrence digamma(x) = digamma(x+n) - sum_{k<n} 1/(x+k) and the asymptotic series, Abramowitz & Stegun 6.3.5,

@@ -1,4 +1,4 @@
-// map.cu -- Stage A on B200: index (host build, HBM resident), per-read mapping kernels, banded
+// map.cu -- Stage A on the GPU: index (host build, HBM resident), per-read mapping kernels, banded
 // affine DP scoring (one warp per mate alignment, lanes = band cells), alignment filtering +
 // auxiliary probabilities + labels, and the equivalence-class builder (hash -> radix sort ->
 // segmented reduce).  C ABI at the reference's seams B1 (processReads, src/quant/
@@ -966,9 +966,9 @@ struct sb_map_ctx {
   uint32_t k1_threads = 0, seed_blocks = 0, dp_blocks = 0;
   BatchBufs b{};                     // cand/score/task buffers: one chunk; outputs: whole batch
   // k_assign of chunk i runs on its own stream next to the seed / DP kernels of chunk i+1 (it is latency-bound at
-  // ~10 % issue utilisation, they are issue-bound): the buffers both sides touch exist twice
+  // low issue utilisation, they are issue-bound): the buffers both sides touch exist twice
   int profile = 0;          // SB_MAP_PROFILE: per-batch host / device times on stderr
-  int overlap_assign = 1;   // +2.7 % at human scale (profiles/stageA_r1_overlap_ab.txt); results bit-identical
+  int overlap_assign = 1;   // results are bit-identical either way
   cudaStream_t assign_stream = nullptr;
   cudaEvent_t ev_dp[2] = {nullptr, nullptr}, ev_asg[2] = {nullptr, nullptr};
   uint32_t *alt_n_l = nullptr, *alt_n_r = nullptr;
@@ -1172,7 +1172,7 @@ extern "C" sb_map_ctx* sb_map_create(sb_index* ix, const sb_map_params* q, int d
   const uint32_t cap = p.max_read_occ;
   const size_t B = batch_cap;
   // reads per pipeline chunk: the per-chunk buffers are sized for chunk_cap; SB_MAP_CHUNK raises it for sweeps
-  size_t chunk_cap = 131072;   // 131072: +4 % over 65536 at human scale (profiles/sweep_r1_stageA_chunk.txt)
+  size_t chunk_cap = 131072;
   if (const char* e = getenv("SB_MAP_CHUNK")) { const long v = atol(e); if (v >= 1024 && v <= (1 << 24)) chunk_cap = (size_t)v; }
   c->chunk = c->chunk_cap = (uint32_t)std::min<size_t>(B, chunk_cap);
   const size_t CH = c->chunk;

@@ -1,4 +1,4 @@
-// map_core.h -- Stage A per-read logic of the product (sm_100a device code; also compiles for
+// map_core.h -- Stage A per-read logic of the product (sm_90a device code; also compiles for
 // the host so that tests can run the SAME code against the independent oracle without a GPU).
 //
 // MAPSPEC (DESIGN.md "Stage A"): seeds sampled every `stride` bases -> hash lookup of the

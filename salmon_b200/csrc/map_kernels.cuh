@@ -1,4 +1,4 @@
-// map_kernels.cuh -- Stage A hot kernels for sm_100a (warp-cooperative forms of MAPSPEC, map_core.h).
+// map_kernels.cuh -- Stage A hot kernels for sm_90a (warp-cooperative forms of MAPSPEC, map_core.h).
 //
 //   k_pack_reads   byte codes -> 2-bit packed reads + N masks (once per batch; both later kernels read 48 B
 //                  per mate instead of L bytes)

@@ -1,7 +1,7 @@
 // pgzip.h -- parallel gzip inflate for the read files (host code, no device work).
 //
 // The reference reads .fastq.gz through kseq/zlib with one inflate thread per file (FQFeeder, pufferfish/external/
-// FastxParser); a single zlib thread delivers ~0.35 GB/s of text, a hundredth of what the mapping kernels take in.
+// FastxParser); a single zlib thread delivers far less text than the mapping kernels take in.
 // Here one gzip file is inflated by several threads:
 //   * BGZF files (bgzip: every member carries its compressed size in a 'BC' extra field): members are independent,
 //     a worker inflates a run of members with zlib;

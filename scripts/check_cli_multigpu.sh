@@ -1,5 +1,5 @@
 #!/bin/bash
-# multi-GPU C++ driver (run with gpurun --gpus N): `sb_salmon quant --gpus N` from reads vs one GPU, and
+# multi-GPU C++ driver (run on a machine with N GPUs): `sb_salmon quant --gpus N` from reads vs one GPU, and
 # `sb_salmon quant -e ... --numBootstraps / --numGibbsSamples --gpus N` (samples split over the GPUs) vs one GPU
 N=${1:-2}
 set -e

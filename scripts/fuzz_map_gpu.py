@@ -1,4 +1,4 @@
-"""Randomised GPU parity (dev helper for the next round, needs a B200): the CUDA mapping path (both kernel variants) against
+"""Randomised GPU parity (dev helper, needs a GPU): the CUDA mapping path (both kernel variants) against
 the oracle over adversarial transcriptomes, read lengths and option settings -- the GPU twin of
 tests/test_map_host.py::test_fuzz_host_logic_against_oracle.  Prints every mismatch, exits 1 if there was one.
 usage: fuzz_map_gpu.py [master_seed] [trials]"""

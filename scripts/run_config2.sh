@@ -1,6 +1,6 @@
 #!/bin/bash
 # BASELINE.json configs[2] as written: human-scale cDNA-only index (synth_txome seed 44, 60000 genes), 20 M synthetic 2x100 bp
-# IU pairs, 1 x B200: `sb_salmon quant` from FASTQ files to quant.sf in ONE timed run.  Files live in /dev/shm.
+# IU pairs, one GPU: `sb_salmon quant` from FASTQ files to quant.sf in ONE timed run.  Files live in /dev/shm.
 set -e
 N=${1:-20000000}
 D=/dev/shm/sb_cfg2; mkdir -p $D/idx gpurun_out

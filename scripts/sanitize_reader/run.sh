@@ -31,7 +31,7 @@ with open(sys.argv[1] + "/t.fa", "w") as f:
 PY
 gzip -k "$W/t_1.fq" "$W/t_2.fq"
 SRC="$HERE/driver.cpp $ROOT/salmon_b200/csrc/ingest.cu $ROOT/salmon_b200/csrc/pipeline.cu $HERE/stubs.cu"
-NV="nvcc -O1 -g -std=c++17 -gencode arch=compute_100a,code=sm_100a"
+NV="nvcc -O1 -g -std=c++17 -gencode arch=compute_90a,code=sm_90a"
 $NV -Xcompiler -fsanitize=thread -Xcompiler -Wno-unknown-pragmas -o "$W/tsan" $SRC -lz -ltsan
 $NV -Xcompiler -fsanitize=address -Xcompiler -fsanitize=undefined -Xcompiler -fopenmp -o "$W/asan" $SRC -lgomp -lz -lasan -lubsan
 echo "== tsan"; TSAN_OPTIONS=halt_on_error=1 "$W/tsan" "$W/t_1.fq" "$W/t_2.fq"

@@ -1,7 +1,7 @@
 """Generates tests/golden/digamma_golden.json with mpmath (50 digits).
 
 Boost.Math (the reference's digamma, CollapsedEMOptimizer.cpp:119,127,256,269) is not
-vendored in /root/reference, so the pin for the oracle's restatement is the function
+vendored in the salmon source tree, so the pin for the oracle's restatement is the function
 itself: high-precision values at seeded points covering every branch (recurrence
 up/down, the [1,2] rational, the x>=10 asymptotic series, the root neighbourhood).
 Run: python tests/golden/make_digamma_golden.py

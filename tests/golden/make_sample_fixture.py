@@ -1,14 +1,14 @@
 """Makes tests/golden/sample_data/ from the reference's bundled sample_data.tgz (BASELINE.json configs[0]: 15 transcripts,
 10 000 simulated 2x50 bp pairs whose names carry the truth, `@<i>:<transcript>:<position>:<fragment length>`).
-Run in the build container (reads /root/reference, which the GPU box does not have); the outputs are committed.
-usage: python tests/golden/make_sample_fixture.py [/root/reference/sample_data.tgz]"""
+Needs a salmon source tree; the outputs are committed, so the tests do not.
+usage: python tests/golden/make_sample_fixture.py <salmon source tree>/sample_data.tgz"""
 import gzip
 import io
 import os
 import sys
 import tarfile
 
-src = sys.argv[1] if len(sys.argv) > 1 else "/root/reference/sample_data.tgz"
+src = sys.argv[1]
 out = os.path.join(os.path.dirname(os.path.abspath(__file__)), "sample_data")
 os.makedirs(out, exist_ok=True)
 with tarfile.open(src) as tf:

@@ -1,49 +1,38 @@
 """The oracle's banded glocal DP recurrence (oracle/map_oracle.c dp_score -- the checker of the CUDA DP kernels) against
-the reference tree's own aligner: edlib (src/edlib.cpp, compiled unmodified into oracle/_ref/libedlib_ref.so by
-oracle/build_ref.sh; salmon uses it for --recoverOrphans).  With unit costs (match 0, mismatch -1, gap open 0, gap extend
-1) the DP's best score is minus the infix (HW) edit distance of the read in the window the band covers, as long as the
-band does not bind -- which holds for random sequences with a few planted edits (an alignment that leaves the band needs
-more indels than the planted distance).  The test skips when oracle/_ref is absent (it is built where /root/reference
-exists and travels with the tree)."""
+the reference tree's own aligner: edlib (src/edlib.cpp; salmon uses it for --recoverOrphans).  With unit costs (match 0,
+mismatch -1, gap open 0, gap extend 1) the DP's best score is minus the infix (HW) edit distance of the read in the window
+the band covers, as long as the band does not bind -- which holds for random sequences with a few planted edits (an
+alignment that leaves the band needs more indels than the planted distance).  edlib's distances for every case are stored
+in tests/golden/edlib_hw.npz, recorded by tests/golden/make_ref_golden.py from edlib compiled unmodified."""
 import ctypes as C
 import os
+import zlib
 
 import numpy as np
-import pytest
 
 import oracle_lib as O
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EDLIB = os.path.join(ROOT, "oracle", "_ref", "libedlib_ref.so")
+GOLDEN = os.path.join(ROOT, "tests", "golden", "edlib_hw.npz")
 
 
-class EdlibAlignConfig(C.Structure):
-    _fields_ = [("k", C.c_int), ("mode", C.c_int), ("task", C.c_int)]
+class _edlib:
+    """edlib's HW distance for the calls test `name` makes, in call order; every call checks that its query and window
+    are the ones the distance was recorded for, and assert_all_used() that no recorded case was left out"""
 
+    def __init__(self, name):
+        g = np.load(GOLDEN)
+        self.name, self.dist, self.crc, self.used = name, g[name + "_d"], g[name + "_crc"], 0
 
-class EdlibAlignResult(C.Structure):
-    _fields_ = [("editDistance", C.c_int), ("endLocations", C.POINTER(C.c_int)), ("startLocations", C.POINTER(C.c_int)),
-                ("numLocations", C.c_int), ("alignment", C.POINTER(C.c_ubyte)), ("alignmentLength", C.c_int),
-                ("alphabetLength", C.c_int)]
+    def __call__(self, query: bytes, target: bytes) -> int:
+        i = self.used
+        assert i < len(self.dist), (self.name, "more calls than recorded cases")
+        assert zlib.crc32(query + b"|" + target) == int(self.crc[i]), (self.name, i)
+        self.used += 1
+        return int(self.dist[i])
 
-
-def _edlib():
-    if not os.path.exists(EDLIB):
-        pytest.skip("oracle/_ref/libedlib_ref.so not built (needs /root/reference)")
-    lib = C.CDLL(EDLIB)
-    align = getattr(lib, "_Z10edlibAlignPKciS0_i16EdlibAlignConfig")      # edlibAlign(const char*, int, const char*, int, EdlibAlignConfig)
-    align.restype = EdlibAlignResult
-    align.argtypes = [C.c_char_p, C.c_int, C.c_char_p, C.c_int, EdlibAlignConfig]
-    free = getattr(lib, "_Z20edlibFreeAlignResult16EdlibAlignResult")
-    free.restype = None
-    free.argtypes = [EdlibAlignResult]
-
-    def hw_distance(query: bytes, target: bytes) -> int:
-        r = align(query, len(query), target, len(target), EdlibAlignConfig(-1, 2, 0))     # k = -1, EDLIB_MODE_HW, TASK_DISTANCE
-        d = r.editDistance
-        free(r)
-        return d
-    return hw_distance
+    def assert_all_used(self):
+        assert self.used == len(self.dist), (self.name, self.used, len(self.dist))
 
 
 def _mutate(rng, s, n_edits):
@@ -61,7 +50,7 @@ def _mutate(rng, s, n_edits):
 
 
 def test_unit_cost_dp_equals_edlib_infix_distance():
-    hw = _edlib()
+    hw = _edlib("unit_cost")
     lib = O.load()
     lib.orc_dp_score.restype = C.c_int32
     rng = np.random.default_rng(41)
@@ -87,12 +76,13 @@ def test_unit_cost_dp_equals_edlib_infix_distance():
         assert score == -d, (trial, L, n_edits, ori, score, d)
         n_checked += 1
     assert n_checked == 1500
+    hw.assert_all_used()
 
 
 def test_default_scores_bound_by_edit_distance():
     """with the default scoring (ma 2, mp -4, go 6, ge 2) an alignment with e edits of the read scores at
     most ma*L (no edits) and at least ma*L - e*(ma + go + ge): edlib's distance brackets the DP score"""
-    hw = _edlib()
+    hw = _edlib("default_scores")
     lib = O.load()
     lib.orc_dp_score.restype = C.c_int32
     rng = np.random.default_rng(43)
@@ -112,6 +102,7 @@ def test_default_scores_bound_by_edit_distance():
         assert p.ma * L - d * worst_per_edit <= score <= p.ma * L - (0 if d == 0 else min(-p.mp + p.ma, p.ge)), (trial, score, d, L)
         if d == 0:
             assert score == p.ma * L
+    hw.assert_all_used()
 
 
 def test_product_serial_dp_equals_edlib_and_oracle():
@@ -119,7 +110,7 @@ def test_product_serial_dp_equals_edlib_and_oracle():
     checked against on the GPU): unit costs against edlib, default scoring against the oracle, same cases"""
     import hostmap_lib
     from salmon_b200._capi import map_default_params
-    hw = _edlib()
+    hw = _edlib("product_serial")
     hl = hostmap_lib.build()
     hl.hmc_dp_score.restype = C.c_int32
     ol = O.load()
@@ -156,6 +147,7 @@ def test_product_serial_dp_equals_edlib_and_oracle():
         if trial % 9 != 0:
             d = hw(letters[read].tobytes(), letters[ref[max(0, diag - B): diag + L + B]].tobytes())
             assert su == -d, (trial, su, d)
+    hw.assert_all_used()
     # reads that hang over either end of the reference: the DP and edlib on the clipped window agree on what is left
     for trial in range(200):
         L = 100

@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): the CUDA EM/VBEM path through the C ABI against the CPU
+"""GPU parity tests (H100): the CUDA EM/VBEM path through the C ABI against the CPU
 oracle on identical inputs.  Tolerances (BASELINE.md section 3):
   combinedWeights / validity flags : bit-exact
   alpha after k iterations          : 1e-9 relative (+1e-9 absolute floor)
@@ -226,7 +226,7 @@ def test_kernel_configurations_agree(ctx, oracle, cfg, rebalance):
     try:
         alpha, st, ok = ctx.optimize(eq, p, proj, eff, uniq)
     finally:
-        ctx.set_option("config", 0); ctx.set_option("rebalance", 1)
+        ctx.set_option("config", 1); ctx.set_option("rebalance", 1)
     ref, rst = oracle.em_optimize(eq, proj, eff, uniq, p)
     assert ok and st.iters == 12
     assert_alpha(alpha, ref)

@@ -527,6 +527,14 @@ int sb_em_debug_timeline(sb_em_ctx* ctx, uint64_t* out, uint32_t iteration);
  *      "blocks_per_sm", "flush_l2_mb". */
 int sb_em_set_option(sb_em_ctx* ctx, const char* key, int64_t value);
 
+/* Figures of the layout sb_em_prepare built (after prepare).  key: "stream_bytes" (bytes one iteration streams:
+ * both SELL matrices at 10 bytes per entry, padding included, + the long rows' CSR at 12), or per matrix with the
+ * suffix "_cm" (class-major) / "_tm" (transcript-major): "stream_bytes", "sell_cols" (SELL columns of 32 entries),
+ * "long_rows", "long_entries", "fallback_rows" (rows on the long-row path only because their slice's indices span
+ * more than 16 bits); "warps" (warps of the iteration grid, which the slice ranges were cut for), "ring_cols"
+ * (columns one warp's stream ring holds). */
+int sb_em_get_info(sb_em_ctx* ctx, const char* key, int64_t* value);
+
 /* ---- multi-GPU: classes stay sharded per rank, alpha is all-reduced once per
  * iteration (the only collective; SURVEY.md section 8e).  The caller provides
  * the NCCL unique id (128 bytes, from sb_nccl_unique_id on rank 0, broadcast

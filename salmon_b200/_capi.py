@@ -183,6 +183,7 @@ SYMBOLS = {
     "sb_em_download": (C.c_int, [_P, _P, C.POINTER(sb_em_stats)]),
     "sb_em_get_combined": (C.c_int, [_P, _P, _P]),
     "sb_em_set_option": (C.c_int, [_P, C.c_char_p, C.c_int64]),
+    "sb_em_get_info": (C.c_int, [_P, C.c_char_p, C.POINTER(C.c_int64)]),
     "sb_em_debug_timeline": (C.c_int, [_P, _P, C.c_uint32]),
     "sb_bootstrap": (C.c_int, [_P, C.POINTER(sb_em_params), C.c_double, C.c_uint32, C.c_uint64, _P, _P]),
     "sb_bootstrap_last_counts": (C.c_int, [_P, _P]),
@@ -375,6 +376,12 @@ class EMContext:
 
     def set_option(self, key: str, value: int):
         _check(self.lib.sb_em_set_option(self.h, key.encode(), int(value)), "sb_em_set_option")
+
+    def info(self, key: str) -> int:
+        """sb_em_get_info: a figure of the prepared layout, e.g. "stream_bytes" or "fallback_rows_tm"."""
+        v = C.c_int64(0)
+        _check(self.lib.sb_em_get_info(self.h, key.encode(), C.byref(v)), "sb_em_get_info")
+        return v.value
 
     @staticmethod
     def _txp_arrays(eq, projected, eff_len, unique):

@@ -22,6 +22,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <string>
 #include <vector>
 
 #include "common.cuh"
@@ -64,8 +65,10 @@ static KernelSet make_set(const char* name) {
   k.p2_partial[1] = k_em_p2_partial<CH, RING, MINB, true>;
   return k;
 }
-// chunk columns x ring depth x resident blocks per SM (shared memory per block = 8 warps x CH x RING x 384 B):
-//   0: 16x2 b2 (96 KB, 16 warps/SM)   1: 8x4 b2   2: 8x3 b3 (72 KB, 24 warps/SM)   3: 8x2 b4 (48 KB, 32 warps/SM)
+// chunk columns x ring depth x resident blocks per SM (shared memory per block = 8 warps x CH x RING x 320 B, a column
+// being 32 x (2-byte index + 8-byte weight)):
+//   0: 16x2 b2 (80 KB, 16 warps/SM)   1: 8x4 b2 (80 KB)   2: 8x3 b3 (60 KB, 24 warps/SM)   3: 8x2 b4 (40 KB, 32 warps/SM)
+// (the resident blocks are capped by the registers the launch bounds allow, not by the shared memory)
 constexpr int N_KERNEL_SETS = 4;
 static const KernelSet& kernel_set(int cfg) {
   static const KernelSet sets[N_KERNEL_SETS] = {
@@ -265,44 +268,73 @@ __global__ void k_remap(uint32_t n, const uint32_t* __restrict__ src,
 }
 
 // ---- CSR -> SELL-32 -------------------------------------------------------------
-// one warp per slice: row lengths, slice width (= max non-long length)
+// one warp per slice: row lengths, slice width (= max non-long length, exact), base index (= smallest gather index of
+// its SELL rows).  A slice whose indices do not fit 16 bits relative to the base (IDX_PAD is reserved) sends its rows
+// to the long-row path (counts: [0] long rows, [2] of which fallback rows).
 __global__ void k_sell_widths(uint32_t n_rows, uint32_t n_slices, uint32_t lmax,
                               const uint32_t* __restrict__ rowperm,
-                              const uint32_t* __restrict__ csr_off, uint16_t* __restrict__ len16,
-                              uint32_t* __restrict__ width, uint32_t* __restrict__ n_long) {
+                              const uint32_t* __restrict__ csr_off, const uint32_t* __restrict__ csr_idx,
+                              uint16_t* __restrict__ len16, uint32_t* __restrict__ width,
+                              uint32_t* __restrict__ sbase, uint32_t* __restrict__ counts) {
   const uint32_t s = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (s >= n_slices) return;
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t row = s * 32 + lane;
-  uint32_t len = 0;
+  uint32_t len = 0, lo = 0xffffffffu, hi = 0;   // len: of a SELL row (0: long or absent)
+  bool sell = false;
   if (row < n_rows) {
     const uint32_t cr = rowperm ? rowperm[row] : row;
-    len = csr_off[cr + 1] - csr_off[cr];
-    if (len > lmax) {
+    const uint32_t b = csr_off[cr];
+    len = csr_off[cr + 1] - b;
+    sell = len <= lmax;
+    if (!sell) {
       len16[row] = LEN_LONG;
-      atomicAdd(n_long, 1u);
+      atomicAdd(&counts[0], 1u);
       len = 0;
-    } else {
-      len16[row] = (uint16_t)len;
+    }
+    for (uint32_t j = 0; j < len; ++j) {
+      lo = min(lo, csr_idx[b + j]);
+      hi = max(hi, csr_idx[b + j]);
     }
   }
-  for (int o = 16; o > 0; o >>= 1) len = max(len, __shfl_xor_sync(0xffffffffu, len, o));
-  if (lane == 0) width[s] = (len + 3u) & ~3u;   // whole column groups of 4 (em_kernels.cuh: run_phase)
+  uint32_t width_s = len;
+  for (int o = 16; o > 0; o >>= 1) {
+    width_s = max(width_s, __shfl_xor_sync(0xffffffffu, width_s, o));
+    lo = min(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+    hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+  }
+  const bool fallback = hi >= lo && hi - lo >= (uint32_t)IDX_PAD;
+  if (sell) {
+    len16[row] = fallback ? LEN_LONG : (uint16_t)len;
+    if (fallback) {
+      atomicAdd(&counts[0], 1u);
+      atomicAdd(&counts[2], 1u);
+    }
+  }
+  if (lane == 0) {
+    width[s] = fallback ? 0u : width_s;
+    sbase[s] = hi >= lo ? lo : 0u;
+  }
 }
 __global__ void k_sell_fill(uint32_t n_rows, uint32_t n_slices, const uint32_t* __restrict__ rowperm,
                             const uint32_t* __restrict__ csr_off, const uint32_t* __restrict__ csr_idx,
                             const double* __restrict__ csr_w, const uint32_t* __restrict__ slice_ptr,
-                            const uint16_t* __restrict__ len16, uint32_t pad_idx,
-                            uint32_t* __restrict__ s_idx, double* __restrict__ s_w,
+                            const uint32_t* __restrict__ sbase, const uint16_t* __restrict__ len16,
+                            uint16_t* __restrict__ s_idx, double* __restrict__ s_w,
                             uint32_t* __restrict__ long_rows, uint32_t* __restrict__ long_cursor) {
   const uint32_t s = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (s >= n_slices) return;
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t row = s * 32 + lane;
-  // group-of-4 layout: entry j of lane l sits at (first column * 32) + (j / 4) * 128 + l * 4 + (j % 4)
-  const size_t base = (size_t)slice_ptr[s] * 32 + (size_t)lane * 4;
+  // entry j of lane l: in the groups of 4 (j < width & ~3) at (first column * 32) + (j / 4) * 128 + l * 4 + (j % 4),
+  // in the remainder columns at (first column + j) * 32 + l (em_kernels.cuh: run_phase)
+  const size_t first = (size_t)slice_ptr[s] * 32;
   const uint32_t width = slice_ptr[s + 1] - slice_ptr[s];
-  auto pos = [&](uint32_t j) { return base + (size_t)(j >> 2) * 128 + (j & 3u); };
+  const uint32_t grouped = width & ~3u;
+  auto pos = [&](uint32_t j) {
+    return j < grouped ? first + (size_t)(j >> 2) * 128 + lane * 4 + (j & 3u) : first + (size_t)j * 32 + lane;
+  };
+  const uint32_t base = sbase[s];
   uint32_t n = 0;
   if (row < n_rows) {
     const uint32_t cr = rowperm ? rowperm[row] : row;
@@ -315,14 +347,14 @@ __global__ void k_sell_fill(uint32_t n_rows, uint32_t n_slices, const uint32_t* 
     } else {
       n = e - b;
       for (uint32_t j = 0; j < n; ++j) {
-        s_idx[pos(j)] = csr_idx[b + j];
+        s_idx[pos(j)] = (uint16_t)(csr_idx[b + j] - base);
         s_w[pos(j)] = csr_w[b + j];
       }
     }
   }
-  // padding: weight 0 and a gather index that always reads 0.0 (slot one past the end)
+  // padding: weight 0 and the index that gathers the zero slot
   for (uint32_t j = n; j < width; ++j) {
-    s_idx[pos(j)] = pad_idx;
+    s_idx[pos(j)] = IDX_PAD;
     s_w[pos(j)] = 0.0;
   }
 }
@@ -519,7 +551,7 @@ extern "C" sb_em_ctx* sb_em_create(int device) {
 }
 
 static void free_sell(SellDev& m) {
-  void** ptrs[] = {(void**)&m.slice_ptr, (void**)&m.width, (void**)&m.len, (void**)&m.idx,
+  void** ptrs[] = {(void**)&m.slice_ptr, (void**)&m.width, (void**)&m.base, (void**)&m.len, (void**)&m.idx,
                    (void**)&m.w, (void**)&m.warp_begin, (void**)&m.long_rows, (void**)&m.targets,
                    };
   for (void** p : ptrs) {
@@ -598,6 +630,34 @@ extern "C" int sb_em_set_option(sb_em_ctx* c, const char* key, int64_t value) {
   else if (!strcmp(key, "overhead_p1")) { c->ovh_p1 = (int)value; c->prepared = false; }
   else if (!strcmp(key, "overhead_p2")) { c->ovh_p2 = (int)value; c->prepared = false; }
   else { set_error("unknown option '%s'", key); return SB_ERR_INVALID; }
+  return SB_OK;
+}
+
+// Figures of the prepared layout (per matrix: suffix _cm = class-major, _tm = transcript-major).
+extern "C" int sb_em_get_info(sb_em_ctx* c, const char* key, int64_t* value) {
+  if (!c || !key || !value) { set_error("null argument"); return SB_ERR_INVALID; }
+  if (!c->prepared) { set_error("sb_em_get_info before sb_em_prepare"); return SB_ERR_STATE; }
+  // bytes one iteration streams: SELL entries (2-byte index + 8-byte weight) and the long rows' CSR (4 + 8 bytes)
+  auto stream = [](const SellDev& m) { return (int64_t)m.n_cols * 32 * 10 + (int64_t)m.long_entries * 12; };
+  if (!strcmp(key, "stream_bytes")) { *value = stream(c->cm) + stream(c->tm); return SB_OK; }
+  // warps of the grid the slice ranges were cut for, and the columns one warp's ring holds
+  if (!strcmp(key, "warps")) { *value = (int64_t)c->grid * (EM_THREADS / 32); return SB_OK; }
+  if (!strcmp(key, "ring_cols")) {
+    const KernelSet& ks = kernel_set(c->config);
+    *value = (int64_t)ks.ch * ks.ring;
+    return SB_OK;
+  }
+  const size_t n = strlen(key);
+  const SellDev* m = nullptr;
+  if (n > 3 && !strcmp(key + n - 3, "_cm")) m = &c->cm;
+  else if (n > 3 && !strcmp(key + n - 3, "_tm")) m = &c->tm;
+  const std::string k(key, m ? n - 3 : n);
+  if (m && k == "stream_bytes") *value = stream(*m);
+  else if (m && k == "sell_cols") *value = m->n_cols;
+  else if (m && k == "long_rows") *value = m->n_long;
+  else if (m && k == "long_entries") *value = (int64_t)m->long_entries;
+  else if (m && k == "fallback_rows") *value = m->n_fallback;
+  else { set_error("unknown info key '%s'", key); return SB_ERR_INVALID; }
   return SB_OK;
 }
 
@@ -683,16 +743,18 @@ static int build_sell(sb_em_ctx* c, SellDev& m, uint32_t n_rows, const uint32_t*
   m.n_slices = (n_rows + 31) / 32;
   m.csr_idx = csr_idx;
   m.csr_w = csr_w;
+  m.zero = pad_idx;
   SB_TRY(dev_alloc(&m.len, (size_t)n_rows));
   SB_TRY(dev_alloc(&m.width, (size_t)m.n_slices + 1));
   SB_TRY(dev_alloc(&m.slice_ptr, (size_t)m.n_slices + 1));
+  SB_TRY(dev_alloc(&m.base, (size_t)m.n_slices + 1));
   SB_TRY(dev_alloc(&m.warp_begin, (size_t)n_warps + 1));
-  uint32_t* d_nlong = (uint32_t*)(c->d_scalars + 8);
-  SB_CUDA(cudaMemsetAsync(d_nlong, 0, 8, st));
+  uint32_t* d_nlong = (uint32_t*)(c->d_scalars + 8);   // [0] long rows, [1] fill cursor, [2] fallback rows
+  SB_CUDA(cudaMemsetAsync(d_nlong, 0, 16, st));
   SB_CUDA(cudaMemsetAsync(m.width, 0, ((size_t)m.n_slices + 1) * 4, st));
   if (m.n_slices) {
-    k_sell_widths<<<nblk(m.n_slices, 8), 256, 0, st>>>(n_rows, m.n_slices, (uint32_t)c->lmax, rowperm, csr_off, m.len,
-                                                       m.width, d_nlong);
+    k_sell_widths<<<nblk(m.n_slices, 8), 256, 0, st>>>(n_rows, m.n_slices, (uint32_t)c->lmax, rowperm, csr_off, csr_idx,
+                                                       m.len, m.width, m.base, d_nlong);
     c->launches++;
   }
   {
@@ -703,20 +765,22 @@ static int build_sell(sb_em_ctx* c, SellDev& m, uint32_t n_rows, const uint32_t*
   uint32_t ncols = 0;
   SB_CUDA(cudaMemcpyAsync(&ncols, m.slice_ptr + m.n_slices, 4, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaMemcpyAsync(&m.n_long, d_nlong, 4, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaMemcpyAsync(&m.n_fallback, d_nlong + 2, 4, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaStreamSynchronize(st));
   m.n_cols = ncols;
   SB_TRY(dev_alloc(&m.idx, (size_t)ncols * 32 + 32));
   SB_TRY(dev_alloc(&m.w, (size_t)ncols * 32 + 32));
   SB_TRY(dev_alloc(&m.long_rows, (size_t)3 * m.n_long + 3));
-  SB_CUDA(cudaMemsetAsync(m.idx, 0, ((size_t)ncols * 32 + 32) * 4, st));
+  SB_CUDA(cudaMemsetAsync(m.idx, 0xff, ((size_t)ncols * 32 + 32) * 2, st));
   SB_CUDA(cudaMemsetAsync(m.w, 0, ((size_t)ncols * 32 + 32) * 8, st));
   if (m.n_slices) {
     k_sell_fill<<<nblk(m.n_slices, 8), 256, 0, st>>>(n_rows, m.n_slices, rowperm, csr_off, csr_idx,
-                                                     csr_w, m.slice_ptr, m.len, pad_idx, m.idx,
+                                                     csr_w, m.slice_ptr, m.base, m.len, m.idx,
                                                      m.w, m.long_rows, d_nlong + 1);
     c->launches++;
   }
   m.n_block = 0;
+  m.long_entries = 0;
   std::vector<uint64_t> h_targets;
   if (m.n_long > 0) {
     // every long row is reduced independently with a fixed tree, so the list order does
@@ -731,8 +795,10 @@ static int build_sell(sb_em_ctx* c, SellDev& m, uint32_t n_rows, const uint32_t*
       const uint32_t lx = h[3 * x + 2] - h[3 * x + 1], ly = h[3 * y + 2] - h[3 * y + 1];
       return lx != ly ? lx > ly : h[3 * x] < h[3 * y];
     });
-    for (uint32_t i = 0; i < m.n_long; ++i)
+    for (uint32_t i = 0; i < m.n_long; ++i) {
       if (h[3 * ord[i] + 2] - h[3 * ord[i] + 1] > (uint32_t)c->lwarp) m.n_block = i + 1;
+      m.long_entries += h[3 * i + 2] - h[3 * i + 1];
+    }
     std::vector<uint32_t> h2(h.size());
     for (uint32_t i = 0; i < m.n_long; ++i)
       for (int k = 0; k < 3; ++k) h2[3 * i + k] = h[3 * ord[i] + k];
@@ -1010,11 +1076,12 @@ extern "C" int sb_em_prepare(sb_em_ctx* c, const sb_em_params* p, sb_em_stats* s
 
 static Sell sell_view(const SellDev& m) {
   Sell s;
-  s.slice_ptr = m.slice_ptr; s.len = m.len; s.idx = m.idx; s.w = m.w; s.warp_begin = m.warp_begin;
+  s.slice_ptr = m.slice_ptr; s.base = m.base; s.len = m.len; s.idx = m.idx; s.w = m.w; s.warp_begin = m.warp_begin;
   s.long_rows = m.long_rows; s.csr_idx = m.csr_idx; s.csr_w = m.csr_w;
   s.n_rows = m.n_rows; s.n_slices = m.n_slices; s.n_long = m.n_long;
   s.n_block = m.n_block;
   s.keep_pct = 100;
+  s.zero = m.zero;
   return s;
 }
 

@@ -12,10 +12,14 @@ namespace sb {
 // Device-side owner of one SELL-32 matrix (see em_kernels.cuh: struct Sell).
 struct SellDev {
   uint32_t n_rows = 0, n_slices = 0, n_cols = 0, n_long = 0, n_block = 0;
+  uint32_t n_fallback = 0;            // rows sent to the long-row path because their slice spans > 16-bit indices
+  uint64_t long_entries = 0;          // entries of all long rows (their CSR copy is what the long-row path reads)
+  uint32_t zero = 0;                  // gather slot holding 0.0 (padding entries)
   uint32_t* slice_ptr = nullptr;
   uint32_t* width = nullptr;
+  uint32_t* base = nullptr;           // per slice: smallest gather index (the 16-bit indices are relative to it)
   uint16_t* len = nullptr;
-  uint32_t* idx = nullptr;
+  uint16_t* idx = nullptr;
   double* w = nullptr;
   uint32_t* warp_begin = nullptr;
   uint32_t* long_rows = nullptr;
@@ -45,7 +49,7 @@ struct sb_em_ctx {
   int sell_group_cm = 1024, sell_group_tm = 1024;   // rows per length-bucketing group (locality window of the gathers)
   int lwarp = 2048;                 // longest row reduced by one warp (longer: one block)
   int balance_long = 0;             // charge the long rows of a warp / block to its share of the slice stream
-  // % of stream chunks pinned in L2 (evict_last).  0 on H100: the ~75 MB of the two layouts at configs[1] size are
+  // % of stream chunks pinned in L2 (evict_last).  0 on H100: the ~67 MB of the two layouts at configs[1] size are
   // well beyond its 50 MB L2, and pinning any share of them measured slower (DESIGN.md section 3.4)
   int keep_cm = 0, keep_tm = 0;
 

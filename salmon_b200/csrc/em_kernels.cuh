@@ -12,9 +12,10 @@
 // Layout: sliced ELL, slice height 32 (SELL-32).  Rows are ordered for gather locality
 // (classes by first transcript id, transcripts by id) and then bucketed by length inside
 // groups of SELL_GROUP rows, so the 32 rows of a slice have (nearly) equal length.  A
-// warp owns a slice: lane = row, entry j of the 32 rows is one coalesced 128-byte (index)
-// + 256-byte (weight) load, each lane accumulates its row sequentially in label order.
-// Slices are dealt to warps in contiguous ranges cut at prepare time -- first by a column
+// warp owns a slice: lane = row, each lane accumulates its row sequentially in label order.
+// A slice is exactly as wide as its longest row; an entry is a 16-bit index relative to the
+// slice's base index + an 8-byte weight, 10 bytes (run_phase has the column order).  A slice
+// whose indices span more than 16 bits hands its rows to the long-row path.  Slices are dealt to warps in contiguous ranges cut at prepare time -- first by a column
 // count model, then re-cut from MEASURED per-warp phase times (em.cu: rebalance).
 // Rows longer than LMAX are reduced by a warp / a whole block from their CSR copy.
 //
@@ -47,13 +48,15 @@ constexpr double DIGAMMA_MIN = 1e-10;        // CollapsedEMOptimizer.cpp:43
 constexpr double MIN_EQ_W = DBL_MIN;         // :40
 constexpr double ALPHA_CHECK_CUTOFF = 1e-2;  // :884
 constexpr uint16_t LEN_LONG = 0xFFFFu;       // row handled by the warp / block path
+constexpr uint16_t IDX_PAD = 0xFFFFu;        // SELL index of a padding entry: gathers the zero slot
 constexpr uint32_t DBG_ACCUMULATE = 0xFFFFFFFFu;   // dbg_it value: accumulate phase durations over all iterations >= 1
 
 // One segmented matrix in SELL-32 form (+ CSR copy of the long rows only).
 struct Sell {
   const uint32_t* slice_ptr;   // [n_slices+1] first column of each slice
+  const uint32_t* base;        // [n_slices] smallest gather index of the slice's SELL rows
   const uint16_t* len;         // [n_rows] entries per row (LEN_LONG: long path)
-  const uint32_t* idx;         // [n_cols*32] gather index, column-interleaved
+  const uint16_t* idx;         // [n_cols*32] gather index - base of the slice (IDX_PAD: padding)
   const double* w;             // [n_cols*32]
   const uint32_t* warp_begin;  // [n_warps+1] slice range per warp
   // long rows: (row, first entry, end entry) triples into csr_idx / csr_w
@@ -63,6 +66,7 @@ struct Sell {
   uint32_t n_rows, n_slices, n_long;
   uint32_t n_block;            // the first n_block long rows (longest first) take the block path
   uint32_t keep_pct;           // % of stream chunks loaded with L2 evict_last (rest evict_first)
+  uint32_t zero;               // gather slot that always holds 0.0 (what padding entries read)
 };
 
 struct EmArgs {
@@ -158,7 +162,7 @@ __device__ __forceinline__ long long block_sum_ll(long long v, double* scratch) 
 template <int CH, int RING>   // CH = columns (x32 entries) per chunk, RING = chunks in flight per warp
 struct __align__(128) WarpRing {
   double w[RING][CH * 32];
-  uint32_t idx[RING][CH * 32];
+  uint16_t idx[RING][CH * 32];
 };
 constexpr int EM_WARPS = EM_THREADS / 32;
 template <int CH, int RING>
@@ -279,9 +283,9 @@ __device__ __forceinline__ void ring_issue(const Sell& S, WarpCtx<CH, RING>& W, 
     // pseudo-random subset of chunks (evict_last) and let the rest stream (evict_first).
     const bool keep = ((((c / CH) * 2654435761u) >> 24) * 100u >> 8) < S.keep_pct;
     const uint64_t pol = keep ? W.pol_keep : W.pol_stream;
-    mbar_arrive_expect_tx(&W.bars[st], cols * 384u);
+    mbar_arrive_expect_tx(&W.bars[st], cols * 320u);
     bulk_g2s_hint(W.ring->w[st], S.w + (size_t)c * 32u, cols * 256u, &W.bars[st], pol);
-    bulk_g2s_hint(W.ring->idx[st], S.idx + (size_t)c * 32u, cols * 128u, &W.bars[st], pol);
+    bulk_g2s_hint(W.ring->idx[st], S.idx + (size_t)c * 32u, cols * 64u, &W.bars[st], pol);
   }
 }
 // fill the ring with the first chunks of a phase.  The matrices are read-only, so this
@@ -303,18 +307,22 @@ __device__ __forceinline__ void ring_drain(WarpCtx<CH, RING>& W, const WarpRange
     if ((uint32_t)k < nchunks) mbar_wait(&W.bars[k], (W.phase_bits >> k) & 1u);
 }
 
-// The SELL stream of a warp.  Columns come in GROUPS of 4 (slice widths are padded to a multiple of 4; padding
-// entries have weight 0 and gather a slot that always holds 0.0): inside a group the layout is lane-major,
+// The SELL stream of a warp.  A slice of width W = its longest row has W / 4 GROUPS of 4 columns and then W % 4
+// remainder columns.  Inside a group the layout is lane-major,
 //   idx[(group * 32 + lane) * 4 + j],  w[(group * 32 + lane) * 4 + j]        j = 0..3,
-// so a lane reads its four indices with ONE 16-byte shared-memory load and its four weights with two, issues the
-// four gathers together and needs no predicate and no remainder loop (a per-column loop with predicated loads needs
-// several times the instructions per column).  Two groups (8 gathers) are in flight when a slice has them.
+// so a lane reads its four indices with ONE 8-byte shared-memory load and its four weights with two 16-byte loads and
+// issues the four gathers together; a remainder column is plain column-major (idx[col * 32 + lane]).  The remainder is
+// the same for the 32 lanes, so it is a warp-uniform branch, not a per-lane predicate.  Padding entries (a row shorter
+// than its slice) have weight 0 and gather a slot that always holds 0.0, so a row's sum is its label-order sum.
+// The ring is a circular buffer of CH * RING columns: column c of the warp's range sits at ring column c % (CH * RING),
+// so a group that straddles two chunks is read in place (each lane's four entries are in one chunk: a chunk boundary
+// falls on a multiple of 32 entries) and a chunk is handed back once the stream has passed its last column.
 template <int PHASE, int CH, int RING, bool VBEM, bool DYNQ, class Deliver>
 __device__ __forceinline__ void run_phase(const EmArgs& A, WarpCtx<CH, RING>& W, const WarpRange& R,
                                           uint32_t bid, uint32_t nblk, double logNorm, double bias,
                                           P2Acc& pa, Deliver&& deliver) {
-  static_assert(CH % 4 == 0, "ring chunks hold whole column groups");
-  constexpr uint32_t CHG = CH / 4;           // groups per chunk
+  static_assert(CH >= 8 && RING >= 2, "two groups in flight span at most two resident chunks");
+  constexpr uint32_t RC = (uint32_t)(CH * RING);   // ring capacity in columns
   const Sell& S = (PHASE == 1) ? A.cm : A.tm;
   // theta / scale are rewritten by other blocks inside the persistent kernel: plain
   // coherent loads only, never ld.global.nc.
@@ -324,73 +332,104 @@ __device__ __forceinline__ void run_phase(const EmArgs& A, WarpCtx<CH, RING>& W,
   const uint32_t s0 = R.s0, s1 = R.s1;
   if (s1 > s0 && R.cend > R.cbeg) {
     const uint32_t nchunks = (R.cend - R.cbeg + CH - 1) / CH;
-    uint32_t rel = 0;                         // groups consumed so far (chunk = rel / CHG)
-    uint32_t sbase = s0;
-    uint32_t sp = (s0 + lane < s1) ? __ldg(&S.slice_ptr[s0 + lane + 1]) : R.cend;   // end columns of 32 slices
-    uint32_t col = R.cbeg;
-    auto fma4 = [&](double& acc, const uint4& i4, const double2& wa, const double2& wb,
-                    double g0, double g1, double g2, double g3) {
-      if (GUARD) {
-        const double v0 = g0 * wa.x, v1 = g1 * wa.y, v2 = g2 * wb.x, v3 = g3 * wb.y;
-        if (!isnan(v0)) acc += v0;
-        if (!isnan(v1)) acc += v1;
-        if (!isnan(v2)) acc += v2;
-        if (!isnan(v3)) acc += v3;
-      } else {
-        acc = fma(g0, wa.x, acc); acc = fma(g1, wa.y, acc); acc = fma(g2, wb.x, acc); acc = fma(g3, wb.y, acc);
+    uint32_t done = 0, ready = 0;             // chunks handed back to the producer / waited for
+    // range columns [c0, c1) resident: hand back the chunks wholly before c0, wait for those up to column c1 - 1
+    auto need = [&](uint32_t c0, uint32_t c1) {
+      for (; (done + 1u) * CH <= c0; ++done) {
+        __syncwarp();
+        if (done + RING < nchunks) ring_issue(S, W, R, done + RING);
+      }
+      for (; ready * CH < c1; ++ready) {
+        const int st = ready % RING;
+        mbar_wait(&W.bars[st], (W.phase_bits >> st) & 1u);
+        W.phase_bits ^= (1u << st);
       }
     };
+    const uint16_t* ri = &W.ring->idx[0][0];
+    const double* rw = &W.ring->w[0][0];
+    // ring entry of this lane's first entry in the group that starts at range column c
+    auto group_at = [&](uint32_t c) {
+      const uint32_t p = (c % RC) * 32u + lane * 4u;
+      return p >= RC * 32u ? p - RC * 32u : p;
+    };
+    auto slot = [&](uint32_t base, uint32_t u) { return u == IDX_PAD ? S.zero : base + u; };
+    auto fma1 = [&](double& acc, double g, double w) {
+      if (GUARD) {
+        const double v = g * w;
+        if (!isnan(v)) acc += v;
+      } else {
+        acc = fma(g, w, acc);
+      }
+    };
+    // one group of four columns: the gathers of the group are issued before any of them is consumed
+    struct Group {
+      double g0, g1, g2, g3;
+      double2 wa, wb;
+    };
+    auto group_load = [&](uint32_t p, uint32_t base) {
+      const uint2 i2 = *reinterpret_cast<const uint2*>(ri + p);
+      Group q;
+      q.g0 = gsrc[slot(base, i2.x & 0xFFFFu)];
+      q.g1 = gsrc[slot(base, i2.x >> 16)];
+      q.g2 = gsrc[slot(base, i2.y & 0xFFFFu)];
+      q.g3 = gsrc[slot(base, i2.y >> 16)];
+      q.wa = *reinterpret_cast<const double2*>(rw + p);
+      q.wb = *reinterpret_cast<const double2*>(rw + p + 2);
+      return q;
+    };
+    auto group_fma = [&](double& acc, const Group& q) {
+      fma1(acc, q.g0, q.wa.x); fma1(acc, q.g1, q.wa.y); fma1(acc, q.g2, q.wb.x); fma1(acc, q.g3, q.wb.y);
+    };
+    uint32_t sbase = s0;
+    uint32_t sp = (s0 + lane < s1) ? __ldg(&S.slice_ptr[s0 + lane + 1]) : R.cend;   // end columns of 32 slices
+    uint32_t sb = (s0 + lane < s1) ? __ldg(&S.base[s0 + lane]) : 0u;                // and their base indices
+    uint32_t c = 0;                           // range column
     RowOps ops_next = load_ops<PHASE>(A, S, s0 * 32u + lane);
     for (uint32_t s = s0; s < s1; ++s) {
       if (s - sbase == 32u) {
         sbase = s;
         sp = (s + lane < s1) ? __ldg(&S.slice_ptr[s + lane + 1]) : R.cend;
+        sb = (s + lane < s1) ? __ldg(&S.base[s + lane]) : 0u;
       }
-      const uint32_t slice_end = __shfl_sync(0xffffffffu, sp, (int)(s - sbase));
-      uint32_t ng = (slice_end - col) >> 2;
-      col = slice_end;
+      const uint32_t slice_end = __shfl_sync(0xffffffffu, sp, (int)(s - sbase)) - R.cbeg;
+      const uint32_t base = __shfl_sync(0xffffffffu, sb, (int)(s - sbase));
+      uint32_t ng = (slice_end - c) >> 2;
+      const uint32_t rem = (slice_end - c) & 3u;
       // epilogue operands one slice ahead: the loads of slice s+1 are in flight while slice s is reduced and finished
       const RowOps ops = ops_next;
       if (s + 1u < s1) ops_next = load_ops<PHASE>(A, S, (s + 1u) * 32u + lane);
-      if (ng == 0) continue;                  // only long / absent rows
+      if (slice_end == c) continue;           // only long / absent rows
       double acc = 0.0;
-      while (ng) {
-        const uint32_t within = rel % CHG;
-        const uint32_t k = rel / CHG;
-        if (within == 0) {                    // entering chunk k: hand back chunk k-1, wait for k
-          if (k > 0) {
-            __syncwarp();
-            if (k - 1u + (uint32_t)RING < nchunks) ring_issue(S, W, R, k - 1u + (uint32_t)RING);
-          }
-          const int st = k % RING;
-          mbar_wait(&W.bars[st], (W.phase_bits >> st) & 1u);
-          W.phase_bits ^= (1u << st);
-        }
-        const int st = k % RING;
-        const uint32_t o = (within * 32u + lane) * 4u;
-        const uint32_t* pi = W.ring->idx[st] + o;
-        const double* pw = W.ring->w[st] + o;
-        if (ng >= 2 && within + 1u < CHG) {   // two groups of this slice in this chunk: 8 gathers in flight
-          const uint4 ia = *reinterpret_cast<const uint4*>(pi);
-          const uint4 ib = *reinterpret_cast<const uint4*>(pi + 128);
-          const double a0 = gsrc[ia.x], a1 = gsrc[ia.y], a2 = gsrc[ia.z], a3 = gsrc[ia.w];
-          const double b0 = gsrc[ib.x], b1 = gsrc[ib.y], b2 = gsrc[ib.z], b3 = gsrc[ib.w];
-          const double2 wa0 = *reinterpret_cast<const double2*>(pw), wa1 = *reinterpret_cast<const double2*>(pw + 2);
-          const double2 wb0 = *reinterpret_cast<const double2*>(pw + 128), wb1 = *reinterpret_cast<const double2*>(pw + 130);
-          fma4(acc, ia, wa0, wa1, a0, a1, a2, a3);
-          fma4(acc, ib, wb0, wb1, b0, b1, b2, b3);
-          rel += 2; ng -= 2;
+      for (; ng >= 2; ng -= 2, c += 8) {      // two groups: 8 gathers in flight
+        need(c, c + 8);
+        const Group qa = group_load(group_at(c), base);
+        const Group qb = group_load(group_at(c + 4), base);
+        group_fma(acc, qa);
+        group_fma(acc, qb);
+      }
+      if (ng) {
+        need(c, c + 4);
+        group_fma(acc, group_load(group_at(c), base));
+        c += 4;
+      }
+      if (rem) {                              // 1-3 remainder columns, column-major
+        need(c, c + rem);
+        const uint32_t p0 = (c % RC) * 32u + lane, p1 = ((c + 1) % RC) * 32u + lane, p2 = ((c + 2) % RC) * 32u + lane;
+        const double g0 = gsrc[slot(base, ri[p0])];
+        if (rem == 1) {
+          fma1(acc, g0, rw[p0]);
+        } else if (rem == 2) {
+          const double g1 = gsrc[slot(base, ri[p1])];
+          fma1(acc, g0, rw[p0]); fma1(acc, g1, rw[p1]);
         } else {
-          const uint4 ia = *reinterpret_cast<const uint4*>(pi);
-          const double a0 = gsrc[ia.x], a1 = gsrc[ia.y], a2 = gsrc[ia.z], a3 = gsrc[ia.w];
-          const double2 wa0 = *reinterpret_cast<const double2*>(pw), wa1 = *reinterpret_cast<const double2*>(pw + 2);
-          fma4(acc, ia, wa0, wa1, a0, a1, a2, a3);
-          rel += 1; ng -= 1;
+          const double g1 = gsrc[slot(base, ri[p1])], g2 = gsrc[slot(base, ri[p2])];
+          fma1(acc, g0, rw[p0]); fma1(acc, g1, rw[p1]); fma1(acc, g2, rw[p2]);
         }
+        c += rem;
       }
       row_finish<PHASE, VBEM>(A, s * 32u + lane, ops, acc, logNorm, bias, pa, deliver);
     }
-    // the last chunk's slot is not re-armed: nothing more to stream in this phase
+    // the chunks still held are not handed back: nothing more to stream in this phase
   }
   if (W.dbg && lane == 0) *W.dbg = gtime_ns();
   if (W.dbg_acc && lane == 0) *W.dbg_acc += gtime_ns() - W.t0;

@@ -30,5 +30,8 @@ for stg in settings:
         continue
     if ref is None:
         ref = a
+    sb = ctx.info("stream_bytes")
     print(f"{str(stg):70s} prepare {st.prepare_ms:6.2f} ms  loop {best / iters * 1e3:7.2f} us/iter  {iters / (best / 1e3):8.0f} iters/s  "
+          f"stream {sb / 1e6:6.2f} MB/iter = {sb * iters / (best / 1e3) / 1e9:6.0f} GB/s  "
+          f"fallback rows {ctx.info('fallback_rows_cm')}/{ctx.info('fallback_rows_tm')}  "
           f"maxdiff vs first {np.max(np.abs(a - ref) / np.maximum(ref, 1e-6)):.1e}", flush=True)

@@ -22,6 +22,12 @@ sizes = (eq.off[1:] - eq.off[:-1]).astype(np.int64)
 tc = np.bincount(eq.tids[np.repeat(sizes > 1, sizes)], minlength=eq.n_txps)
 print("classes >32:", int((sizes > 32).sum()), " txps >32:", int((tc > 32).sum()), ">256:", int((tc > 256).sum()), ">2048:", int((tc > 2048).sum()), "max", int(tc.max()), " entries in txp rows >32:", int(tc[tc > 32].sum()))
 print("C", C, "loop us/iter", r.loop_kernel_ms / 60 * 1e3, "warps", nw)
+sb = ctx.info("stream_bytes")
+print("stream per iteration: %.2f MB (class-major %.2f, transcript-major %.2f; SELL columns %d / %d; long-row entries %d / %d; "
+      "fallback rows %d / %d) = %.0f GB/s" % (
+          sb / 1e6, ctx.info("stream_bytes_cm") / 1e6, ctx.info("stream_bytes_tm") / 1e6, ctx.info("sell_cols_cm"),
+          ctx.info("sell_cols_tm"), ctx.info("long_entries_cm"), ctx.info("long_entries_tm"), ctx.info("fallback_rows_cm"),
+          ctx.info("fallback_rows_tm"), sb / (r.loop_kernel_ms / 60 * 1e-3) / 1e9))
 for i, n in enumerate(names):
     col = t[:, i] - t0
     print(f"{n:11s} min {col.min()/1e3:8.2f}  p50 {np.median(col)/1e3:8.2f}  p90 {np.percentile(col,90)/1e3:8.2f}  max {col.max()/1e3:8.2f} us")

@@ -470,7 +470,7 @@ class EMContext:
         return _check(self.lib.sb_em_debug_timeline(self.h, None, iteration), "sb_em_debug_timeline")
 
     def read_timeline(self, n_warps: int):
-        out = np.zeros((n_warps, 8), dtype=np.uint64)
+        out = np.zeros((n_warps, 16), dtype=np.uint64)   # DBG_SLOTS (em_kernels.cuh: SB_DBG)
         _check(self.lib.sb_em_debug_timeline(self.h, out.ctypes.data, 0), "sb_em_debug_timeline")
         return out
 

@@ -552,7 +552,8 @@ extern "C" sb_em_ctx* sb_em_create(int device) {
 
 static void free_sell(SellDev& m) {
   void** ptrs[] = {(void**)&m.slice_ptr, (void**)&m.width, (void**)&m.base, (void**)&m.len, (void**)&m.idx,
-                   (void**)&m.w, (void**)&m.warp_begin, (void**)&m.long_rows, (void**)&m.targets,
+                   (void**)&m.w, (void**)&m.warp_begin, (void**)&m.home_end, (void**)&m.long_rows, (void**)&m.tiles,
+                   (void**)&m.targets,
                    };
   for (void** p : ptrs) {
     if (*p) cudaFree(*p);
@@ -627,6 +628,13 @@ extern "C" int sb_em_set_option(sb_em_ctx* c, const char* key, int64_t value) {
   else if (!strcmp(key, "sample_offset")) { c->sample_offset = (uint32_t)value; }
   else if (!strcmp(key, "rebalance")) { c->rebalance = (int)value; c->prepared = false; }
   else if (!strcmp(key, "rebalance_iters")) { c->rebalance_iters = (int)value; c->prepared = false; }
+  else if (!strcmp(key, "tail_pct")) {
+    if (value < 0 || value > 100) { set_error("tail_pct out of range"); return SB_ERR_INVALID; }
+    c->tail_pct = (int)value; c->prepared = false;
+  } else if (!strcmp(key, "tail_tile_cols")) {
+    if (value < 1 || value > 65536) { set_error("tail_tile_cols out of range"); return SB_ERR_INVALID; }
+    c->tail_tile_cols = (int)value; c->prepared = false;
+  }
   else if (!strcmp(key, "overhead_p1")) { c->ovh_p1 = (int)value; c->prepared = false; }
   else if (!strcmp(key, "overhead_p2")) { c->ovh_p2 = (int)value; c->prepared = false; }
   else { set_error("unknown option '%s'", key); return SB_ERR_INVALID; }
@@ -657,6 +665,9 @@ extern "C" int sb_em_get_info(sb_em_ctx* c, const char* key, int64_t* value) {
   else if (m && k == "long_rows") *value = m->n_long;
   else if (m && k == "long_entries") *value = (int64_t)m->long_entries;
   else if (m && k == "fallback_rows") *value = m->n_fallback;
+  else if (m && k == "tail_tiles") *value = m->n_tiles;
+  else if (m && k == "tail_cols") *value = (int64_t)m->tail_cols;
+  else if (m && k == "home_cols") *value = (int64_t)m->home_cols;
   else { set_error("unknown info key '%s'", key); return SB_ERR_INVALID; }
   return SB_OK;
 }
@@ -731,6 +742,55 @@ static int scan_u64(sb_em_ctx* c, const uint64_t* in, uint64_t* out, uint64_t n)
   size_t tb = c->tmp_bytes;
   SB_CUDA(cub::DeviceScan::ExclusiveSum(c->d_tmp, tb, in, out, (int)n, c->stream));
   c->launches += 2;
+  return SB_OK;
+}
+
+// modelled cost of a slice in columns: its width plus the epilogue overhead (slices of long rows only cost nothing)
+static double slice_cost(const std::vector<uint32_t>& sp, uint32_t s, uint32_t overhead) {
+  return (double)(sp[s + 1] - sp[s]) + (sp[s + 1] > sp[s] ? (double)overhead : 0.0);
+}
+
+// Split every warp's slice range [s0, s1) at h: the home part [s0, h) carries (100 - tail_pct) % of the range's
+// modelled work and streams through the warp's ring; [h, s1) is cut at slice boundaries into tail tiles of at least
+// tail_tile_cols columns (a shorter rest joins the warp's previous tile), which the phase's work queue hands to
+// whichever warp is free after the long rows.  Every slice lies in exactly one home part or one tile.
+static int split_tails(sb_em_ctx* c, SellDev& m, uint32_t overhead, uint32_t n_warps) {
+  std::vector<uint32_t> sp((size_t)m.n_slices + 1), wb((size_t)n_warps + 1), home(std::max<uint32_t>(n_warps, 1));
+  SB_CUDA(cudaMemcpy(sp.data(), m.slice_ptr, sp.size() * 4, cudaMemcpyDeviceToHost));
+  SB_CUDA(cudaMemcpy(wb.data(), m.warp_begin, wb.size() * 4, cudaMemcpyDeviceToHost));
+  std::vector<uint4> tiles;
+  m.home_cols = m.tail_cols = 0;
+  for (uint32_t w = 0; w < n_warps; ++w) {
+    const uint32_t s0 = wb[w], s1 = wb[w + 1];
+    uint32_t h = s1;
+    if (c->tail_pct > 0) {
+      double work = 0.0;
+      for (uint32_t s = s0; s < s1; ++s) work += slice_cost(sp, s, overhead);
+      const double target = work * (100 - c->tail_pct) / 100.0;
+      double cum = 0.0;
+      for (h = s0; h < s1 && cum + 0.5 * slice_cost(sp, h, overhead) < target; ++h) cum += slice_cost(sp, h, overhead);
+    }
+    home[w] = h;
+    m.home_cols += sp[h] - sp[s0];
+    m.tail_cols += sp[s1] - sp[h];
+    const size_t first = tiles.size();
+    for (uint32_t t0 = h; t0 < s1;) {
+      uint32_t t1 = t0 + 1;
+      while (t1 < s1 && sp[t1] - sp[t0] < (uint32_t)c->tail_tile_cols) ++t1;
+      if (sp[t1] - sp[t0] < (uint32_t)c->tail_tile_cols && tiles.size() > first) {
+        tiles.back().y = t1;                   // a short rest joins the previous tile
+        tiles.back().w = sp[t1];
+      } else {
+        tiles.push_back(make_uint4(t0, t1, sp[t0], sp[t1]));
+      }
+      t0 = t1;
+    }
+  }
+  m.n_tiles = (uint32_t)tiles.size();
+  SB_TRY(dev_alloc(&m.home_end, home.size()));
+  SB_TRY(dev_alloc(&m.tiles, tiles.size()));
+  SB_CUDA(cudaMemcpy(m.home_end, home.data(), home.size() * 4, cudaMemcpyHostToDevice));
+  if (!tiles.empty()) SB_CUDA(cudaMemcpy(m.tiles, tiles.data(), tiles.size() * sizeof(uint4), cudaMemcpyHostToDevice));
   return SB_OK;
 }
 
@@ -842,7 +902,7 @@ static int build_sell(sb_em_ctx* c, SellDev& m, uint32_t n_rows, const uint32_t*
                                                         m.warp_begin);
   c->launches++;
   SB_CUDA(cudaStreamSynchronize(st));   // h_targets must outlive the copy
-  return SB_OK;
+  return split_tails(c, m, overhead, n_warps);
 }
 
 static int em_rebalance(sb_em_ctx* c);
@@ -1077,8 +1137,10 @@ extern "C" int sb_em_prepare(sb_em_ctx* c, const sb_em_params* p, sb_em_stats* s
 static Sell sell_view(const SellDev& m) {
   Sell s;
   s.slice_ptr = m.slice_ptr; s.base = m.base; s.len = m.len; s.idx = m.idx; s.w = m.w; s.warp_begin = m.warp_begin;
+  s.home_end = m.home_end;
   s.long_rows = m.long_rows; s.csr_idx = m.csr_idx; s.csr_w = m.csr_w;
-  s.n_rows = m.n_rows; s.n_slices = m.n_slices; s.n_long = m.n_long;
+  s.tiles = m.tiles;
+  s.n_rows = m.n_rows; s.n_slices = m.n_slices; s.n_long = m.n_long; s.n_tiles = m.n_tiles;
   s.n_block = m.n_block;
   s.keep_pct = 100;
   s.zero = m.zero;
@@ -1538,23 +1600,28 @@ static int em_recut(sb_em_ctx* c, sb::SellDev& m, uint32_t overhead, const std::
   const uint32_t n_warps = n_warps_all / unit;        // ranges
   if (m.n_slices == 0 || n_warps == 0) return SB_OK;
   std::vector<uint32_t> sp((size_t)m.n_slices + 1), wb_all((size_t)n_warps_all + 1), wb((size_t)n_warps + 1);
+  std::vector<uint32_t> home_all((size_t)n_warps_all);
   SB_CUDA(cudaMemcpy(sp.data(), m.slice_ptr, sp.size() * 4, cudaMemcpyDeviceToHost));
   SB_CUDA(cudaMemcpy(wb_all.data(), m.warp_begin, wb_all.size() * 4, cudaMemcpyDeviceToHost));
-  std::vector<unsigned long long> dbg((size_t)n_warps * 8, 0ull);
+  SB_CUDA(cudaMemcpy(home_all.data(), m.home_end, home_all.size() * 4, cudaMemcpyDeviceToHost));
+  std::vector<unsigned long long> dbg((size_t)n_warps * DBG_SLOTS, 0ull);
   for (uint32_t r = 0; r <= n_warps; ++r) wb[r] = wb_all[(size_t)r * unit];
   for (uint32_t r = 0; r < n_warps; ++r)
-    for (int k = 0; k < 8; ++k) {
+    for (uint32_t k = 0; k < DBG_SLOTS; ++k) {
       unsigned long long a = 0;
-      for (uint32_t u = 0; u < unit; ++u) a += dbg_w[((size_t)r * unit + u) * 8 + k];
-      dbg[(size_t)r * 8 + k] = a / unit;
+      for (uint32_t u = 0; u < unit; ++u) a += dbg_w[((size_t)r * unit + u) * DBG_SLOTS + k];
+      dbg[(size_t)r * DBG_SLOTS + k] = a / unit;
     }
-  auto cost = [&](uint32_t s) { return (double)(sp[s + 1] - sp[s]) + (sp[s + 1] > sp[s] ? (double)overhead : 0.0); };
+  auto cost = [&](uint32_t s) { return slice_cost(sp, s, overhead); };
   std::vector<double> fixed(n_warps), dens(n_warps, 0.0);
   double sell_total = 0.0, dens_sum = 0.0, work_sum = 0.0;
   for (uint32_t w = 0; w < n_warps; ++w) {
-    const double T = (double)dbg[(size_t)w * 8 + slot_total], Ts = std::min(T, (double)dbg[(size_t)w * 8 + slot_sell]);
+    // the SELL tap fires at the end of the home stream: the density is home-part time over home-part work
+    const double T = (double)dbg[(size_t)w * DBG_SLOTS + slot_total];
+    const double Ts = std::min(T, (double)dbg[(size_t)w * DBG_SLOTS + slot_sell]);
     double W = 0.0;
-    for (uint32_t s = wb[w]; s < wb[w + 1]; ++s) W += cost(s);
+    for (uint32_t u = 0; u < unit; ++u)
+      for (uint32_t s = wb_all[(size_t)w * unit + u]; s < home_all[(size_t)w * unit + u]; ++s) W += cost(s);
     fixed[w] = 0.0 * (T - Ts);   // the long rows are taken from a global queue: every warp's tail is filled, nothing is fixed
     if (W > 0.0) { dens[w] = Ts / W; dens_sum += Ts; work_sum += W; }
     sell_total += Ts;
@@ -1603,8 +1670,8 @@ static int em_recut(sb_em_ctx* c, sb::SellDev& m, uint32_t overhead, const std::
 
 static int em_rebalance(sb_em_ctx* c) {
   const uint32_t n_warps = c->grid * (EM_THREADS / 32);
-  SB_TRY(dev_alloc(&c->d_dbg, (size_t)n_warps * 8));
-  SB_CUDA(cudaMemsetAsync(c->d_dbg, 0, (size_t)n_warps * 64, c->stream));
+  SB_TRY(dev_alloc(&c->d_dbg, (size_t)n_warps * DBG_SLOTS));
+  SB_CUDA(cudaMemsetAsync(c->d_dbg, 0, (size_t)n_warps * DBG_SLOTS * 8, c->stream));
   const sb_em_params saved = c->params;
   const uint32_t saved_it = c->dbg_it;
   const bool saved_en = c->dbg_enabled;
@@ -1614,11 +1681,14 @@ static int em_rebalance(sb_em_ctx* c) {
   int rc = sb_em_run(c, nullptr);
   c->params = saved; c->dbg_it = saved_it; c->dbg_enabled = saved_en;
   if (rc != SB_OK) return rc;
-  std::vector<unsigned long long> dbg((size_t)n_warps * 8);
+  std::vector<unsigned long long> dbg((size_t)n_warps * DBG_SLOTS);
   SB_CUDA(cudaMemcpy(dbg.data(), c->d_dbg, dbg.size() * 8, cudaMemcpyDeviceToHost));
   const uint32_t unit = 1u;
+  const uint32_t ovh_tm = (uint32_t)(c->params.use_vbem ? c->ovh_p2 : c->ovh_p1);
   SB_TRY(em_recut(c, c->cm, (uint32_t)c->ovh_p1, dbg, 0, 3, n_warps, unit));
-  SB_TRY(em_recut(c, c->tm, (uint32_t)(c->params.use_vbem ? c->ovh_p2 : c->ovh_p1), dbg, 1, 4, n_warps, unit));
+  SB_TRY(em_recut(c, c->tm, ovh_tm, dbg, 1, 4, n_warps, unit));
+  SB_TRY(split_tails(c, c->cm, (uint32_t)c->ovh_p1, n_warps));
+  SB_TRY(split_tails(c, c->tm, ovh_tm, n_warps));
   return SB_OK;
 }
 
@@ -1693,14 +1763,14 @@ extern "C" int sb_em_debug_timeline(sb_em_ctx* c, uint64_t* out, uint32_t iterat
   const uint32_t n_warps = c->grid * (EM_THREADS / 32);
   if (!out) {
     // arm: the next sb_em_run records iteration `iteration`
-    SB_TRY(dev_alloc(&c->d_dbg, (size_t)n_warps * 8));
-    SB_CUDA(cudaMemset(c->d_dbg, 0, (size_t)n_warps * 64));
+    SB_TRY(dev_alloc(&c->d_dbg, (size_t)n_warps * DBG_SLOTS));
+    SB_CUDA(cudaMemset(c->d_dbg, 0, (size_t)n_warps * DBG_SLOTS * 8));
     c->dbg_it = iteration;
     c->dbg_enabled = true;
     return (int)n_warps;
   }
   if (!c->d_dbg) { set_error("timeline not armed"); return SB_ERR_STATE; }
-  SB_CUDA(cudaMemcpy(out, c->d_dbg, (size_t)n_warps * 64, cudaMemcpyDeviceToHost));
+  SB_CUDA(cudaMemcpy(out, c->d_dbg, (size_t)n_warps * DBG_SLOTS * 8, cudaMemcpyDeviceToHost));
   return (int)n_warps;
 }
 

@@ -16,15 +16,16 @@
 // A slice is exactly as wide as its longest row; an entry is a 16-bit index relative to the
 // slice's base index + an 8-byte weight, 10 bytes (run_phase has the column order).  A slice
 // whose indices span more than 16 bits hands its rows to the long-row path.  Slices are dealt to warps in contiguous ranges cut at prepare time -- first by a column
-// count model, then re-cut from MEASURED per-warp phase times (em.cu: rebalance).
+// count model, then re-cut from MEASURED per-warp phase times (em.cu: rebalance).  Optionally the last tail_pct % of each
+// range's modelled work is cut off as TAIL TILES (em.cu: split_tails), which go on the phase's work queue after the
+// long rows (off by default: a tile reduced from global memory measured slower than the ring path).
 // Rows longer than LMAX are reduced by a warp / a whole block from their CSR copy.
 //
 // Design points (a warp's time goes to waiting at the grid barriers, L2 gather latency and dependent FP64 chains):
-//   * the consumption loop is software-pipelined over BATCHES of <= NB columns: the gathers of
-//     batch b+1 (and the epilogue operands of its slice) are issued before batch b is consumed
-//     and before the epilogue of a finished slice runs, so a slice costs max(gather round trip,
-//     epilogue chain) instead of their sum, and a short slice is ONE round trip (not a 4-wide batch
-//     plus one serialised round trip per remaining column);
+//   * a warp streams its home range through its ring, then takes long rows (and tail tiles) from one queue until it
+//     is empty.  Every SELL row is summed by one lane in label order, wherever it is reduced;
+//   * inside a slice the gathers of two groups of 4 columns are issued before either is consumed, and the epilogue
+//     operands of slice s+1 are loaded while slice s is reduced (gathers are not pipelined across slices);
 //   * the VBEM epilogue is one branch-light function (em_math.h) instead of a Boost-style
 //     digamma with data-dependent loops followed by exp();
 //   * VBEM / EM are template parameters: the NaN guard of plain EM (:206) is compiled out of VBEM;
@@ -50,6 +51,7 @@ constexpr double ALPHA_CHECK_CUTOFF = 1e-2;  // :884
 constexpr uint16_t LEN_LONG = 0xFFFFu;       // row handled by the warp / block path
 constexpr uint16_t IDX_PAD = 0xFFFFu;        // SELL index of a padding entry: gathers the zero slot
 constexpr uint32_t DBG_ACCUMULATE = 0xFFFFFFFFu;   // dbg_it value: accumulate phase durations over all iterations >= 1
+constexpr uint32_t DBG_SLOTS = 16;                  // timeline slots per warp (see SB_DBG)
 
 // One segmented matrix in SELL-32 form (+ CSR copy of the long rows only).
 struct Sell {
@@ -59,11 +61,14 @@ struct Sell {
   const uint16_t* idx;         // [n_cols*32] gather index - base of the slice (IDX_PAD: padding)
   const double* w;             // [n_cols*32]
   const uint32_t* warp_begin;  // [n_warps+1] slice range per warp
+  const uint32_t* home_end;    // [n_warps] end of the warp's home part, streamed through its ring; the rest of its
+                               // range is tail tiles
   // long rows: (row, first entry, end entry) triples into csr_idx / csr_w
   const uint32_t* long_rows;   // [3*n_long]
   const uint32_t* csr_idx;
   const double* csr_w;
-  uint32_t n_rows, n_slices, n_long;
+  const uint4* tiles;          // [n_tiles] tail tiles: (first slice, end slice, first column, end column)
+  uint32_t n_rows, n_slices, n_long, n_tiles;
   uint32_t n_block;            // the first n_block long rows (longest first) take the block path
   uint32_t keep_pct;           // % of stream chunks loaded with L2 evict_last (rest evict_first)
   uint32_t zero;               // gather slot that always holds 0.0 (what padding entries read)
@@ -89,9 +94,9 @@ struct EmArgs {
   double first_bias;            // 1.0 for optimize's first plain-EM iteration (:812,:821), else 0
   uint32_t min_iter, max_iter;
   uint32_t* out;                // [0]=iters [1]=converged [2]=maxrel slot
-  unsigned long long* dbg;      // optional [n_warps*8] phase timestamps (ns) of iteration dbg_it
+  unsigned long long* dbg;      // optional [n_warps*DBG_SLOTS] phase timestamps (ns) of iteration dbg_it
   uint32_t dbg_it;
-  unsigned int* lq;             // [2] global long-row queues of the persistent kernels (P1, P2)
+  unsigned int* lq;             // [2] work queues (long rows, then tail tiles) of the persistent kernels (P1, P2)
   // multi-GPU, fused exchange over peer memory (k_em_persistent_mgpu): every rank owns one exchange block (layout:
   // XchgLayout) mapped into every peer (CUDA IPC, NVLink P2P)
   unsigned char* const* peers;  // [nranks] base pointers of the exchange blocks (peers[rank] = own)
@@ -175,7 +180,7 @@ struct WarpCtx {
   uint32_t phase_bits;   // mbarrier parity per stage
   double* scratch;       // block scratch (40 doubles)
   uint64_t pol_keep, pol_stream;   // L2 eviction policies of the bulk copies
-  unsigned long long* dbg;  // optional: timestamp after the SELL part of a phase
+  unsigned long long* dbg;  // optional: the warp's timeline row (end of the home stream, queue items taken)
   unsigned long long* dbg_acc;   // optional: accumulates (end of the SELL part - t0)
   unsigned long long t0;
 };
@@ -261,14 +266,14 @@ __device__ __forceinline__ void row_finish(const EmArgs& A, uint32_t row, const 
   }
 }
 
-// static stream range of one warp in one matrix (the matrices never change)
+// static home stream range of one warp in one matrix (the matrices never change)
 struct WarpRange {
   uint32_t s0, s1, cbeg, cend;
 };
 __device__ __forceinline__ WarpRange load_range(const Sell& S, uint32_t gwarp) {
   WarpRange r;
   r.s0 = __ldg(&S.warp_begin[gwarp]);
-  r.s1 = __ldg(&S.warp_begin[gwarp + 1]);
+  r.s1 = __ldg(&S.home_end[gwarp]);
   r.cbeg = __ldg(&S.slice_ptr[r.s0]);
   r.cend = __ldg(&S.slice_ptr[r.s1]);
   return r;
@@ -307,132 +312,187 @@ __device__ __forceinline__ void ring_drain(WarpCtx<CH, RING>& W, const WarpRange
     if ((uint32_t)k < nchunks) mbar_wait(&W.bars[k], (W.phase_bits >> k) & 1u);
 }
 
-// The SELL stream of a warp.  A slice of width W = its longest row has W / 4 GROUPS of 4 columns and then W % 4
-// remainder columns.  Inside a group the layout is lane-major,
+// Where sell_rows reads the entries of column c, counted from the first column of the slices it reduces.  A slice of
+// width W = its longest row has W / 4 GROUPS of 4 columns and then W % 4 remainder columns.  Inside a group the layout
+// is lane-major,
 //   idx[(group * 32 + lane) * 4 + j],  w[(group * 32 + lane) * 4 + j]        j = 0..3,
-// so a lane reads its four indices with ONE 8-byte shared-memory load and its four weights with two 16-byte loads and
-// issues the four gathers together; a remainder column is plain column-major (idx[col * 32 + lane]).  The remainder is
-// the same for the 32 lanes, so it is a warp-uniform branch, not a per-lane predicate.  Padding entries (a row shorter
-// than its slice) have weight 0 and gather a slot that always holds 0.0, so a row's sum is its label-order sum.
-// The ring is a circular buffer of CH * RING columns: column c of the warp's range sits at ring column c % (CH * RING),
-// so a group that straddles two chunks is read in place (each lane's four entries are in one chunk: a chunk boundary
-// falls on a multiple of 32 entries) and a chunk is handed back once the stream has passed its last column.
-template <int PHASE, int CH, int RING, bool VBEM, bool DYNQ, class Deliver>
-__device__ __forceinline__ void run_phase(const EmArgs& A, WarpCtx<CH, RING>& W, const WarpRange& R,
-                                          uint32_t bid, uint32_t nblk, double logNorm, double bias,
-                                          P2Acc& pa, Deliver&& deliver) {
-  static_assert(CH >= 8 && RING >= 2, "two groups in flight span at most two resident chunks");
-  constexpr uint32_t RC = (uint32_t)(CH * RING);   // ring capacity in columns
-  const Sell& S = (PHASE == 1) ? A.cm : A.tm;
+// so a lane reads its four indices with ONE 8-byte load and its four weights with two 16-byte loads and issues the
+// four gathers together; a remainder column is plain column-major (idx[col * 32 + lane]).
+//
+// RingCols: a warp's home range, streamed through its TMA ring.  The ring is a circular buffer of CH * RING columns:
+// column c sits at ring column c % (CH * RING), so a group that straddles two chunks is read in place (each lane's four
+// entries are in one chunk: a chunk boundary falls on a multiple of 32 entries) and a chunk is handed back once the
+// stream has passed its last column.
+template <int CH, int RING>
+struct RingCols {
+  static constexpr uint32_t RC = (uint32_t)(CH * RING);   // ring capacity in columns
+  const Sell& S;
+  WarpCtx<CH, RING>& W;
+  const WarpRange& R;
+  uint32_t lane, nchunks;
+  uint32_t done = 0, ready = 0;             // chunks handed back to the producer / waited for
+  // columns [c0, c1) resident: hand back the chunks wholly before c0, wait for those up to column c1 - 1
+  __device__ __forceinline__ void need(uint32_t c0, uint32_t c1) {
+    for (; (done + 1u) * CH <= c0; ++done) {
+      __syncwarp();
+      if (done + RING < nchunks) ring_issue(S, W, R, done + RING);
+    }
+    for (; ready * CH < c1; ++ready) {
+      const int st = ready % RING;
+      mbar_wait(&W.bars[st], (W.phase_bits >> st) & 1u);
+      W.phase_bits ^= (1u << st);
+    }
+  }
+  // ring entry of this lane's first entry in the group that starts at column c
+  __device__ __forceinline__ uint32_t group_at(uint32_t c) const {
+    const uint32_t p = (c % RC) * 32u + lane * 4u;
+    return p >= RC * 32u ? p - RC * 32u : p;
+  }
+  __device__ __forceinline__ uint2 idx4(uint32_t c) const {
+    return *reinterpret_cast<const uint2*>(&W.ring->idx[0][0] + group_at(c));
+  }
+  __device__ __forceinline__ double2 w4(uint32_t c, uint32_t j) const {
+    return *reinterpret_cast<const double2*>(&W.ring->w[0][0] + group_at(c) + j);
+  }
+  __device__ __forceinline__ uint32_t idx1(uint32_t c) const { return (&W.ring->idx[0][0])[(c % RC) * 32u + lane]; }
+  __device__ __forceinline__ double w1(uint32_t c) const { return (&W.ring->w[0][0])[(c % RC) * 32u + lane]; }
+};
+// GlobalCols: a tail tile, read straight from the layout in global memory
+struct GlobalCols {
+  const uint16_t* idx;   // the tile's first column
+  const double* w;
+  uint32_t lane;
+  __device__ __forceinline__ void need(uint32_t, uint32_t) const {}
+  __device__ __forceinline__ uint2 idx4(uint32_t c) const {
+    return __ldg(reinterpret_cast<const uint2*>(idx + c * 32u + lane * 4u));
+  }
+  __device__ __forceinline__ double2 w4(uint32_t c, uint32_t j) const {
+    return __ldg(reinterpret_cast<const double2*>(w + c * 32u + lane * 4u + j));
+  }
+  __device__ __forceinline__ uint32_t idx1(uint32_t c) const { return __ldg(idx + c * 32u + lane); }
+  __device__ __forceinline__ double w1(uint32_t c) const { return __ldg(w + c * 32u + lane); }
+};
+
+// The rows of slices [s0, s1), whose columns are [cbeg, cend) of the layout, read through `cols`.  Every row is summed
+// by one lane in label order -- pairs of groups (8 gathers in flight), then a single group, then the remainder columns
+// -- and finished (row_finish) with operands loaded one slice ahead.  The ring path and the tail-tile path both call
+// this, so a row's sum does not depend on which path reduced it.  The remainder is the same for the 32 lanes, so it is
+// a warp-uniform branch, not a per-lane predicate.  Padding entries (a row shorter than its slice) have weight 0 and
+// gather a slot that always holds 0.0, so a row's sum is its label-order sum.
+template <int PHASE, bool VBEM, class Cols, class Deliver>
+__device__ __forceinline__ void sell_rows(const EmArgs& A, const Sell& S, Cols& cols, uint32_t s0, uint32_t s1,
+                                          uint32_t cbeg, uint32_t cend, double logNorm, double bias, P2Acc& pa,
+                                          Deliver&& deliver) {
   // theta / scale are rewritten by other blocks inside the persistent kernel: plain
   // coherent loads only, never ld.global.nc.
   const double* gsrc = (PHASE == 1) ? A.theta : A.scale;
   constexpr bool GUARD = (PHASE == 1) && !VBEM;   // plain EM skips NaN products (:206)
   const uint32_t lane = threadIdx.x & 31u;
-  const uint32_t s0 = R.s0, s1 = R.s1;
-  if (s1 > s0 && R.cend > R.cbeg) {
-    const uint32_t nchunks = (R.cend - R.cbeg + CH - 1) / CH;
-    uint32_t done = 0, ready = 0;             // chunks handed back to the producer / waited for
-    // range columns [c0, c1) resident: hand back the chunks wholly before c0, wait for those up to column c1 - 1
-    auto need = [&](uint32_t c0, uint32_t c1) {
-      for (; (done + 1u) * CH <= c0; ++done) {
-        __syncwarp();
-        if (done + RING < nchunks) ring_issue(S, W, R, done + RING);
-      }
-      for (; ready * CH < c1; ++ready) {
-        const int st = ready % RING;
-        mbar_wait(&W.bars[st], (W.phase_bits >> st) & 1u);
-        W.phase_bits ^= (1u << st);
-      }
-    };
-    const uint16_t* ri = &W.ring->idx[0][0];
-    const double* rw = &W.ring->w[0][0];
-    // ring entry of this lane's first entry in the group that starts at range column c
-    auto group_at = [&](uint32_t c) {
-      const uint32_t p = (c % RC) * 32u + lane * 4u;
-      return p >= RC * 32u ? p - RC * 32u : p;
-    };
-    auto slot = [&](uint32_t base, uint32_t u) { return u == IDX_PAD ? S.zero : base + u; };
-    auto fma1 = [&](double& acc, double g, double w) {
-      if (GUARD) {
-        const double v = g * w;
-        if (!isnan(v)) acc += v;
-      } else {
-        acc = fma(g, w, acc);
-      }
-    };
-    // one group of four columns: the gathers of the group are issued before any of them is consumed
-    struct Group {
-      double g0, g1, g2, g3;
-      double2 wa, wb;
-    };
-    auto group_load = [&](uint32_t p, uint32_t base) {
-      const uint2 i2 = *reinterpret_cast<const uint2*>(ri + p);
-      Group q;
-      q.g0 = gsrc[slot(base, i2.x & 0xFFFFu)];
-      q.g1 = gsrc[slot(base, i2.x >> 16)];
-      q.g2 = gsrc[slot(base, i2.y & 0xFFFFu)];
-      q.g3 = gsrc[slot(base, i2.y >> 16)];
-      q.wa = *reinterpret_cast<const double2*>(rw + p);
-      q.wb = *reinterpret_cast<const double2*>(rw + p + 2);
-      return q;
-    };
-    auto group_fma = [&](double& acc, const Group& q) {
-      fma1(acc, q.g0, q.wa.x); fma1(acc, q.g1, q.wa.y); fma1(acc, q.g2, q.wb.x); fma1(acc, q.g3, q.wb.y);
-    };
-    uint32_t sbase = s0;
-    uint32_t sp = (s0 + lane < s1) ? __ldg(&S.slice_ptr[s0 + lane + 1]) : R.cend;   // end columns of 32 slices
-    uint32_t sb = (s0 + lane < s1) ? __ldg(&S.base[s0 + lane]) : 0u;                // and their base indices
-    uint32_t c = 0;                           // range column
-    RowOps ops_next = load_ops<PHASE>(A, S, s0 * 32u + lane);
-    for (uint32_t s = s0; s < s1; ++s) {
-      if (s - sbase == 32u) {
-        sbase = s;
-        sp = (s + lane < s1) ? __ldg(&S.slice_ptr[s + lane + 1]) : R.cend;
-        sb = (s + lane < s1) ? __ldg(&S.base[s + lane]) : 0u;
-      }
-      const uint32_t slice_end = __shfl_sync(0xffffffffu, sp, (int)(s - sbase)) - R.cbeg;
-      const uint32_t base = __shfl_sync(0xffffffffu, sb, (int)(s - sbase));
-      uint32_t ng = (slice_end - c) >> 2;
-      const uint32_t rem = (slice_end - c) & 3u;
-      // epilogue operands one slice ahead: the loads of slice s+1 are in flight while slice s is reduced and finished
-      const RowOps ops = ops_next;
-      if (s + 1u < s1) ops_next = load_ops<PHASE>(A, S, (s + 1u) * 32u + lane);
-      if (slice_end == c) continue;           // only long / absent rows
-      double acc = 0.0;
-      for (; ng >= 2; ng -= 2, c += 8) {      // two groups: 8 gathers in flight
-        need(c, c + 8);
-        const Group qa = group_load(group_at(c), base);
-        const Group qb = group_load(group_at(c + 4), base);
-        group_fma(acc, qa);
-        group_fma(acc, qb);
-      }
-      if (ng) {
-        need(c, c + 4);
-        group_fma(acc, group_load(group_at(c), base));
-        c += 4;
-      }
-      if (rem) {                              // 1-3 remainder columns, column-major
-        need(c, c + rem);
-        const uint32_t p0 = (c % RC) * 32u + lane, p1 = ((c + 1) % RC) * 32u + lane, p2 = ((c + 2) % RC) * 32u + lane;
-        const double g0 = gsrc[slot(base, ri[p0])];
-        if (rem == 1) {
-          fma1(acc, g0, rw[p0]);
-        } else if (rem == 2) {
-          const double g1 = gsrc[slot(base, ri[p1])];
-          fma1(acc, g0, rw[p0]); fma1(acc, g1, rw[p1]);
-        } else {
-          const double g1 = gsrc[slot(base, ri[p1])], g2 = gsrc[slot(base, ri[p2])];
-          fma1(acc, g0, rw[p0]); fma1(acc, g1, rw[p1]); fma1(acc, g2, rw[p2]);
-        }
-        c += rem;
-      }
-      row_finish<PHASE, VBEM>(A, s * 32u + lane, ops, acc, logNorm, bias, pa, deliver);
+  auto slot = [&](uint32_t base, uint32_t u) { return u == IDX_PAD ? S.zero : base + u; };
+  auto fma1 = [&](double& acc, double g, double w) {
+    if (GUARD) {
+      const double v = g * w;
+      if (!isnan(v)) acc += v;
+    } else {
+      acc = fma(g, w, acc);
     }
+  };
+  // one group of four columns: the gathers of the group are issued before any of them is consumed
+  struct Group {
+    double g0, g1, g2, g3;
+    double2 wa, wb;
+  };
+  auto group_load = [&](uint32_t c, uint32_t base) {
+    const uint2 i2 = cols.idx4(c);
+    Group q;
+    q.g0 = gsrc[slot(base, i2.x & 0xFFFFu)];
+    q.g1 = gsrc[slot(base, i2.x >> 16)];
+    q.g2 = gsrc[slot(base, i2.y & 0xFFFFu)];
+    q.g3 = gsrc[slot(base, i2.y >> 16)];
+    q.wa = cols.w4(c, 0u);
+    q.wb = cols.w4(c, 2u);
+    return q;
+  };
+  auto group_fma = [&](double& acc, const Group& q) {
+    fma1(acc, q.g0, q.wa.x); fma1(acc, q.g1, q.wa.y); fma1(acc, q.g2, q.wb.x); fma1(acc, q.g3, q.wb.y);
+  };
+  uint32_t sbase = s0;
+  uint32_t sp = (s0 + lane < s1) ? __ldg(&S.slice_ptr[s0 + lane + 1]) : cend;   // end columns of 32 slices
+  uint32_t sb = (s0 + lane < s1) ? __ldg(&S.base[s0 + lane]) : 0u;              // and their base indices
+  uint32_t c = 0;                           // column, counted from cbeg
+  RowOps ops_next = load_ops<PHASE>(A, S, s0 * 32u + lane);
+  for (uint32_t s = s0; s < s1; ++s) {
+    if (s - sbase == 32u) {
+      sbase = s;
+      sp = (s + lane < s1) ? __ldg(&S.slice_ptr[s + lane + 1]) : cend;
+      sb = (s + lane < s1) ? __ldg(&S.base[s + lane]) : 0u;
+    }
+    const uint32_t slice_end = __shfl_sync(0xffffffffu, sp, (int)(s - sbase)) - cbeg;
+    const uint32_t base = __shfl_sync(0xffffffffu, sb, (int)(s - sbase));
+    uint32_t ng = (slice_end - c) >> 2;
+    const uint32_t rem = (slice_end - c) & 3u;
+    // epilogue operands one slice ahead: the loads of slice s+1 are in flight while slice s is reduced and finished
+    const RowOps ops = ops_next;
+    if (s + 1u < s1) ops_next = load_ops<PHASE>(A, S, (s + 1u) * 32u + lane);
+    if (slice_end == c) continue;           // only long / absent rows
+    double acc = 0.0;
+    for (; ng >= 2; ng -= 2, c += 8) {      // two groups: 8 gathers in flight
+      cols.need(c, c + 8);
+      const Group qa = group_load(c, base);
+      const Group qb = group_load(c + 4, base);
+      group_fma(acc, qa);
+      group_fma(acc, qb);
+    }
+    if (ng) {
+      cols.need(c, c + 4);
+      group_fma(acc, group_load(c, base));
+      c += 4;
+    }
+    if (rem) {                              // 1-3 remainder columns, column-major
+      cols.need(c, c + rem);
+      const double g0 = gsrc[slot(base, cols.idx1(c))];
+      if (rem == 1) {
+        fma1(acc, g0, cols.w1(c));
+      } else if (rem == 2) {
+        const double g1 = gsrc[slot(base, cols.idx1(c + 1))];
+        fma1(acc, g0, cols.w1(c)); fma1(acc, g1, cols.w1(c + 1));
+      } else {
+        const double g1 = gsrc[slot(base, cols.idx1(c + 1))], g2 = gsrc[slot(base, cols.idx1(c + 2))];
+        fma1(acc, g0, cols.w1(c)); fma1(acc, g1, cols.w1(c + 1)); fma1(acc, g2, cols.w1(c + 2));
+      }
+      c += rem;
+    }
+    row_finish<PHASE, VBEM>(A, s * 32u + lane, ops, acc, logNorm, bias, pa, deliver);
+  }
+}
+
+struct Nothing {
+  __device__ __forceinline__ void operator()() const {}
+};
+
+// One phase of a warp: its home range through the ring, then `after_home` (the ring is idle from there on: the caller
+// hands it to the next phase's home range), then the block-path rows, then the phase's work queue.  Queue items
+// [0, n_mid) are the long rows (LMAX < len <= LWARP), longest first; items [n_mid, n_mid + n_tiles) are the tail
+// tiles.  Big items first, small ones fill the end.
+template <int PHASE, int CH, int RING, bool VBEM, bool DYNQ, class AfterHome, class Deliver>
+__device__ __forceinline__ void run_phase(const EmArgs& A, WarpCtx<CH, RING>& W, const WarpRange& R,
+                                          uint32_t bid, uint32_t nblk, double logNorm, double bias,
+                                          P2Acc& pa, AfterHome&& after_home, Deliver&& deliver) {
+  static_assert(CH >= 8 && RING >= 2, "two groups in flight span at most two resident chunks");
+  const Sell& S = (PHASE == 1) ? A.cm : A.tm;
+  const double* gsrc = (PHASE == 1) ? A.theta : A.scale;
+  constexpr bool GUARD = (PHASE == 1) && !VBEM;   // plain EM skips NaN products (:206)
+  const uint32_t lane = threadIdx.x & 31u;
+  if (R.s1 > R.s0 && R.cend > R.cbeg) {
+    RingCols<CH, RING> rc{S, W, R, lane, (R.cend - R.cbeg + CH - 1) / CH};
+    sell_rows<PHASE, VBEM>(A, S, rc, R.s0, R.s1, R.cbeg, R.cend, logNorm, bias, pa, deliver);
     // the chunks still held are not handed back: nothing more to stream in this phase
   }
-  if (W.dbg && lane == 0) *W.dbg = gtime_ns();
+  unsigned long long* const dbg = W.dbg;
+  if (dbg && lane == 0) dbg[PHASE == 1 ? 8 : 7] = gtime_ns();
   if (W.dbg_acc && lane == 0) *W.dbg_acc += gtime_ns() - W.t0;
+  __syncwarp();   // every lane has read its last ring entry before lane 0 refills the ring
+  after_home();
   // very long rows: whole block per row, fixed-order tree reduction
   for (uint32_t li = bid; li < S.n_block; li += nblk) {
     const uint32_t r = __ldg(&S.long_rows[3 * li]);
@@ -464,17 +524,16 @@ __device__ __forceinline__ void run_phase(const EmArgs& A, WarpCtx<CH, RING>& W,
     }
     __syncthreads();
   }
-  // long rows (LMAX < len <= LWARP): one warp per row, lanes stride the CSR copy with four independent gathers in
-  // flight, fixed shuffle tree.  Sorted longest-first.  Persistent kernels (DYNQ): taken one at a time from a global
-  // queue by whichever warp has finished its SELL share (the next claim is in flight while a row is reduced), so the
-  // tail of a phase is filled evenly -- dealt round-robin, the warp that draws the longest row ends the phase well
-  // after the others.  Per-phase launches: dealt round-robin over the warps of the grid.
+  // The work queue.  Persistent kernels (DYNQ): items are taken one at a time from a global queue by whichever warp is
+  // free (the next claim is in flight while an item is reduced), so the tail of a phase is filled evenly -- dealt
+  // statically, the warp that draws the longest row ends the phase well after the others.  Claiming two ahead measured
+  // slower: the first free warp took the two longest rows.  Per-phase launches: dealt round-robin over the warps.
   {
     const uint32_t gw = bid * EM_WARPS + (threadIdx.x >> 5);
     const uint32_t nw = nblk * EM_WARPS;
-    const uint32_t n_mid = S.n_long - S.n_block;
+    const uint32_t n_mid = S.n_long - S.n_block, n_items = n_mid + S.n_tiles;
     unsigned int* queue = A.lq + ((PHASE == 1) ? 0 : 1);
-    // lane k keeps the sum of the k-th row this warp reduced; the epilogues (digamma, exp)
+    // lane k keeps the sum of the k-th long row this warp reduced; the epilogues (digamma, exp)
     // then run lane-parallel, 32 rows at a time.
     uint32_t cnt = 0, myrow = 0xffffffffu;
     double myacc = 0.0;
@@ -492,50 +551,89 @@ __device__ __forceinline__ void run_phase(const EmArgs& A, WarpCtx<CH, RING>& W,
       if (lane == 0) q = atomicAdd(queue, 1u);
       return q;               // lane 0's value is broadcast when it is consumed
     };
-    uint32_t q_next = 0;
-    if (DYNQ) { if (n_mid) q_next = claim(); } else q_next = gw;
+    // an item: (row, first entry, end entry) of a long row, or (first slice, end slice, first column, end column) of a
+    // tail tile
+    auto item = [&](uint32_t q) {
+      uint4 d = make_uint4(0u, 0u, 0u, 0u);
+      if (q < n_mid) {
+        const uint32_t li = S.n_block + q;
+        d.x = __ldg(&S.long_rows[3 * li]);
+        d.y = __ldg(&S.long_rows[3 * li + 1]);
+        d.z = __ldg(&S.long_rows[3 * li + 2]);
+      } else if (q < n_items) {
+        d = __ldg(&S.tiles[q - n_mid]);
+      }
+      return d;
+    };
+    uint32_t q_next;
+    if (DYNQ) q_next = n_items ? claim() : 0u; else q_next = gw;
+    // timeline: what this warp took from the queue (slots zeroed when the timeline is armed)
+    unsigned long long* const qs = (dbg && lane == 0) ? dbg + (PHASE == 1 ? 9 : 12) : nullptr;
     for (;;) {
-      uint32_t q = DYNQ ? __shfl_sync(0xffffffffu, q_next, 0) : q_next;
-      if (q >= n_mid) break;
+      const uint32_t q = DYNQ ? __shfl_sync(0xffffffffu, q_next, 0) : q_next;
+      if (q >= n_items) break;
       if (DYNQ) q_next = claim(); else q_next = q + nw;
-      const uint32_t li = S.n_block + q;
-      const uint32_t r = __ldg(&S.long_rows[3 * li]);
-      const uint32_t b = __ldg(&S.long_rows[3 * li + 1]);
-      const uint32_t e = __ldg(&S.long_rows[3 * li + 2]);
-      double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
-      uint32_t k = b + lane;
-      for (; k + 96 < e; k += 128) {
-        const uint32_t i0 = __ldg(&S.csr_idx[k]), i1 = __ldg(&S.csr_idx[k + 32]);
-        const uint32_t i2 = __ldg(&S.csr_idx[k + 64]), i3 = __ldg(&S.csr_idx[k + 96]);
-        const double g0 = gsrc[i0], g1 = gsrc[i1], g2 = gsrc[i2], g3 = gsrc[i3];
-        double v0 = g0 * __ldg(&S.csr_w[k]), v1 = g1 * __ldg(&S.csr_w[k + 32]);
-        double v2 = g2 * __ldg(&S.csr_w[k + 64]), v3 = g3 * __ldg(&S.csr_w[k + 96]);
-        if (GUARD) {
-          if (isnan(v0)) v0 = 0.0;
-          if (isnan(v1)) v1 = 0.0;
-          if (isnan(v2)) v2 = 0.0;
-          if (isnan(v3)) v3 = 0.0;
+      const uint4 d = item(q);
+      if (q < n_mid) {
+        // one warp per row, lanes stride the CSR copy with four independent gathers in flight, fixed shuffle tree.
+        // The CSR loads of step k + 128 are issued before the gathers of step k are consumed.
+        const uint32_t r = d.x, b = d.y, e = d.z;
+        double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
+        uint32_t k = b + lane;
+        uint32_t i0 = 0u, i1 = 0u, i2 = 0u, i3 = 0u;
+        double w0 = 0.0, w1 = 0.0, w2 = 0.0, w3 = 0.0;
+        if (k + 96 < e) {
+          i0 = __ldg(&S.csr_idx[k]); i1 = __ldg(&S.csr_idx[k + 32]);
+          i2 = __ldg(&S.csr_idx[k + 64]); i3 = __ldg(&S.csr_idx[k + 96]);
+          w0 = __ldg(&S.csr_w[k]); w1 = __ldg(&S.csr_w[k + 32]);
+          w2 = __ldg(&S.csr_w[k + 64]); w3 = __ldg(&S.csr_w[k + 96]);
         }
-        a0 += v0; a1 += v1; a2 += v2; a3 += v3;
-      }
-      {
-        // tail: up to three more strides, issued together
-        const uint32_t i0 = (k < e) ? __ldg(&S.csr_idx[k]) : 0u;
-        const uint32_t i1 = (k + 32 < e) ? __ldg(&S.csr_idx[k + 32]) : 0u;
-        const uint32_t i2 = (k + 64 < e) ? __ldg(&S.csr_idx[k + 64]) : 0u;
-        double v0 = (k < e) ? gsrc[i0] * __ldg(&S.csr_w[k]) : 0.0;
-        double v1 = (k + 32 < e) ? gsrc[i1] * __ldg(&S.csr_w[k + 32]) : 0.0;
-        double v2 = (k + 64 < e) ? gsrc[i2] * __ldg(&S.csr_w[k + 64]) : 0.0;
-        if (GUARD) {
-          if (isnan(v0)) v0 = 0.0;
-          if (isnan(v1)) v1 = 0.0;
-          if (isnan(v2)) v2 = 0.0;
+        for (; k + 96 < e; k += 128) {
+          const double g0 = gsrc[i0], g1 = gsrc[i1], g2 = gsrc[i2], g3 = gsrc[i3];
+          const double x0 = w0, x1 = w1, x2 = w2, x3 = w3;
+          // no branch around the next step's loads (a last step reloads its own entries), so that they can be issued
+          // ahead of this step's FMAs
+          const uint32_t kn = (k + 224 < e) ? k + 128 : k;
+          i0 = __ldg(&S.csr_idx[kn]); i1 = __ldg(&S.csr_idx[kn + 32]);
+          i2 = __ldg(&S.csr_idx[kn + 64]); i3 = __ldg(&S.csr_idx[kn + 96]);
+          w0 = __ldg(&S.csr_w[kn]); w1 = __ldg(&S.csr_w[kn + 32]);
+          w2 = __ldg(&S.csr_w[kn + 64]); w3 = __ldg(&S.csr_w[kn + 96]);
+          double v0 = g0 * x0, v1 = g1 * x1;
+          double v2 = g2 * x2, v3 = g3 * x3;
+          if (GUARD) {
+            if (isnan(v0)) v0 = 0.0;
+            if (isnan(v1)) v1 = 0.0;
+            if (isnan(v2)) v2 = 0.0;
+            if (isnan(v3)) v3 = 0.0;
+          }
+          a0 += v0; a1 += v1; a2 += v2; a3 += v3;
         }
-        a0 += v0; a1 += v1; a2 += v2;
+        {
+          // tail: up to three more strides, issued together
+          const uint32_t j0 = (k < e) ? __ldg(&S.csr_idx[k]) : 0u;
+          const uint32_t j1 = (k + 32 < e) ? __ldg(&S.csr_idx[k + 32]) : 0u;
+          const uint32_t j2 = (k + 64 < e) ? __ldg(&S.csr_idx[k + 64]) : 0u;
+          double v0 = (k < e) ? gsrc[j0] * __ldg(&S.csr_w[k]) : 0.0;
+          double v1 = (k + 32 < e) ? gsrc[j1] * __ldg(&S.csr_w[k + 32]) : 0.0;
+          double v2 = (k + 64 < e) ? gsrc[j2] * __ldg(&S.csr_w[k + 64]) : 0.0;
+          if (GUARD) {
+            if (isnan(v0)) v0 = 0.0;
+            if (isnan(v1)) v1 = 0.0;
+            if (isnan(v2)) v2 = 0.0;
+          }
+          a0 += v0; a1 += v1; a2 += v2;
+        }
+        const double acc = warp_sum((a0 + a1) + (a2 + a3));
+        if (lane == cnt) { myacc = acc; myrow = r; }
+        if (++cnt == 32) flush();
+        if (qs) { qs[0] += (1ull << 32) | (e - b); qs[2] = max(qs[2], (unsigned long long)(e - b)); }
+      } else {
+        if (d.w > d.z) {
+          GlobalCols gc{S.idx + (size_t)d.z * 32u, S.w + (size_t)d.z * 32u, lane};
+          sell_rows<PHASE, VBEM>(A, S, gc, d.x, d.y, d.z, d.w, logNorm, bias, pa, deliver);
+        }
+        if (qs) qs[1] += (1ull << 32) | (d.w - d.z);
       }
-      const double acc = warp_sum((a0 + a1) + (a2 + a3));
-      if (lane == cnt) { myacc = acc; myrow = r; }
-      if (++cnt == 32) flush();
     }
     flush();
   }
@@ -584,15 +682,18 @@ __device__ __forceinline__ void p2_finish(const EmArgs& A, double* scratch, P2Ac
 
 // timeline taps: one iteration's timestamps (dbg_it = that iteration), or phase durations accumulated over the
 // iterations >= 1 of a run (dbg_it = DBG_ACCUMULATE; slot 0 = P1, slot 1 = P2, slot 2 = iterations) -- the input of
-// the measured re-balancing in em.cu (slots 3 / 4: the SELL part of P1 / P2 alone)
+// the measured re-balancing in em.cu (slots 3 / 4: the home stream of P1 / P2 alone).  One iteration's row of the
+// persistent kernel: 0 P1 start, 1 P1 end, 2 end of barrier 1, 3 P2 start, 4 P2 end, 5 reduction end, 6 end of
+// barrier 2, 7 / 8 end of the P2 / P1 home stream, 9-11 / 12-14 what the warp took from the P1 / P2 queue:
+// (long rows << 32 | their entries), (tail tiles << 32 | their columns), longest row taken (run_phase)
 #define SB_DBG(slot)                                                        \
-  if (A.dbg && it == A.dbg_it && (threadIdx.x & 31u) == 0) A.dbg[(size_t)gwarp * 8 + (slot)] = gtime_ns();
+  if (A.dbg && it == A.dbg_it && (threadIdx.x & 31u) == 0) A.dbg[(size_t)gwarp * DBG_SLOTS + (slot)] = gtime_ns();
 #define SB_ACC_BEGIN(var, sell_slot) \
   unsigned long long var = 0; \
-  if (dbg_acc) { var = gtime_ns(); W.t0 = var; W.dbg_acc = &A.dbg[(size_t)gwarp * 8 + (sell_slot)]; }
+  if (dbg_acc) { var = gtime_ns(); W.t0 = var; W.dbg_acc = &A.dbg[(size_t)gwarp * DBG_SLOTS + (sell_slot)]; }
 #define SB_ACC_END(var, slot) \
   W.dbg_acc = nullptr; \
-  if (dbg_acc && (threadIdx.x & 31u) == 0) A.dbg[(size_t)gwarp * 8 + (slot)] += gtime_ns() - var;
+  if (dbg_acc && (threadIdx.x & 31u) == 0) A.dbg[(size_t)gwarp * DBG_SLOTS + (slot)] += gtime_ns() - var;
 
 // ---- persistent cooperative kernel: the whole iteration loop, two grid barriers/iter
 template <int CH, int RING, int MINB, bool VBEM>
@@ -618,29 +719,30 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent(const __grid
     P2Acc pa{0ll, 0.0};
     SB_DBG(0)
     SB_ACC_BEGIN(t1, 3)
-    run_phase<1, CH, RING, VBEM, true>(A, W, R1, bid, nblk, 0.0, 0.0, pa, NoDeliver{});
+    W.dbg = (A.dbg && it == A.dbg_it) ? &A.dbg[(size_t)gwarp * DBG_SLOTS] : nullptr;
+    // P2's home stream lands while this warp takes queue items and during the grid barrier
+    run_phase<1, CH, RING, VBEM, true>(A, W, R1, bid, nblk, 0.0, 0.0, pa, [&] { ring_prefetch(A.tm, W, R2); }, NoDeliver{});
     SB_ACC_END(t1, 0)
     SB_DBG(1)
-    ring_prefetch(A.tm, W, R2);   // P2's stream lands during the grid barrier
     grid.sync();
     SB_DBG(2)
-    if (bid == 0 && threadIdx.x == 0) A.lq[0] = 0u;   // P1's long-row queue: idle until the next iteration
+    if (bid == 0 && threadIdx.x == 0) A.lq[0] = 0u;   // P1's work queue: idle until the next iteration
     if (VBEM && it > 0) logNorm = scratch[33];   // written before the grid barrier above
     const double bias = (it == 0) ? A.first_bias : 0.0;  // alphasPrime starts at 1.0 (:812,:821)
     SB_DBG(3)
     SB_ACC_BEGIN(t2, 4)
-    W.dbg = (A.dbg && it == A.dbg_it) ? &A.dbg[(size_t)gwarp * 8 + 7] : nullptr;
-    run_phase<2, CH, RING, VBEM, true>(A, W, R2, bid, nblk, logNorm, bias, pa, NoDeliver{});
+    // next iteration's P1 home stream (harmless if the loop ends)
+    run_phase<2, CH, RING, VBEM, true>(A, W, R2, bid, nblk, logNorm, bias, pa, [&] { ring_prefetch(A.cm, W, R1); },
+                                       NoDeliver{});
     W.dbg = nullptr;
     SB_ACC_END(t2, 1)
     SB_DBG(4)
-    ring_prefetch(A.cm, W, R1);   // next iteration's P1 stream (harmless if the loop ends)
     p2_finish(A, scratch, pa, par);
     SB_DBG(5)
     grid.sync();
     SB_DBG(6)
-    if (bid == 0 && threadIdx.x == 0) A.lq[1] = 0u;   // P2's long-row queue
-    if (dbg_acc && (threadIdx.x & 31u) == 0) A.dbg[(size_t)gwarp * 8 + 2] += 1ull;
+    if (bid == 0 && threadIdx.x == 0) A.lq[1] = 0u;   // P2's work queue
+    if (dbg_acc && (threadIdx.x & 31u) == 0) A.dbg[(size_t)gwarp * DBG_SLOTS + 2] += 1ull;
     const double mr = __longlong_as_double((long long)__ldcg(&A.maxrel[par]));
     converged = !(mr > A.tol);
     ++it;
@@ -777,10 +879,9 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent_mgpu(const _
     P2Acc pa{0ll, 0.0};
     SB_DBG(0)
     SB_ACC_BEGIN(t1, 3)
-    run_phase<1, CH, RING, VBEM, true>(A, W, R1, bid, nblk, 0.0, 0.0, pa, NoDeliver{});
+    run_phase<1, CH, RING, VBEM, true>(A, W, R1, bid, nblk, 0.0, 0.0, pa, [&] { ring_prefetch(A.tm, W, R2); }, NoDeliver{});
     SB_ACC_END(t1, 0)
     SB_DBG(1)
-    ring_prefetch(A.tm, W, R2);
     grid.sync();
     SB_DBG(2)
     if (bid == 0 && threadIdx.x == 0) A.lq[0] = 0u;
@@ -788,10 +889,10 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent_mgpu(const _
     if (A.push_pass) {
       // this rank's share of alpha' per transcript id into the local buffer (locally inactive transcripts keep their
       // constant folded singleton mass, written once per run by the host) ...
-      run_phase<3, CH, RING, VBEM, true>(A, W, R2, bid, nblk, 0.0, 0.0, pa, DeliverLocal{A.part_out});
+      run_phase<3, CH, RING, VBEM, true>(A, W, R2, bid, nblk, 0.0, 0.0, pa, [&] { ring_prefetch(A.cm, W, R1); },
+                                         DeliverLocal{A.part_out});
       SB_ACC_END(t2, 1)
       SB_DBG(3)
-      ring_prefetch(A.cm, W, R1);
       __threadfence();
       grid.sync();
       if (bid == 0 && threadIdx.x == 0) A.lq[1] = 0u;
@@ -805,10 +906,9 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent_mgpu(const _
       // straight from the row epilogues; locally inactive transcripts (constant share) first
       for (uint32_t t = gtid; t < M; t += gthreads)
         if (__ldg(&A.tid_row[t]) == 0xffffffffu) push(t, __ldg(&A.base[t]));
-      run_phase<3, CH, RING, VBEM, true>(A, W, R2, bid, nblk, 0.0, 0.0, pa, push);
+      run_phase<3, CH, RING, VBEM, true>(A, W, R2, bid, nblk, 0.0, 0.0, pa, [&] { ring_prefetch(A.cm, W, R1); }, push);
       SB_ACC_END(t2, 1)
       SB_DBG(3)
-      ring_prefetch(A.cm, W, R1);
     }
     // ---- owner phase: my slice [lo, hi); the lines are polled as they arrive
     const double bias = (it == 0) ? A.first_bias : 0.0;
@@ -900,7 +1000,7 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent_mgpu(const _
       if (VBEM) logNorm = digamma_pos(__ldcg(&A.sum_partial[par]));
     }
     SB_DBG(7)
-    if (dbg_acc && (threadIdx.x & 31u) == 0) A.dbg[(size_t)gwarp * 8 + 2] += 1ull;
+    if (dbg_acc && (threadIdx.x & 31u) == 0) A.dbg[(size_t)gwarp * DBG_SLOTS + 2] += 1ull;
     ++it;
   }
   // all-gather of the final alpha: every owner pushes its slice into every rank's alpha region
@@ -927,7 +1027,7 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_p1(const __grid_constan
   P2Acc pa{0ll, 0.0};
   const WarpRange R = load_range(A.cm, blockIdx.x * (EM_THREADS / 32) + (threadIdx.x >> 5));
   ring_prefetch(A.cm, W, R);
-  run_phase<1, CH, RING, VBEM, false>(A, W, R, blockIdx.x, gridDim.x, 0.0, 0.0, pa, NoDeliver{});
+  run_phase<1, CH, RING, VBEM, false>(A, W, R, blockIdx.x, gridDim.x, 0.0, 0.0, pa, Nothing{}, NoDeliver{});
 }
 template <int CH, int RING, int MINB, bool VBEM>
 __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_p2(const __grid_constant__ EmArgs A, uint32_t it) {
@@ -950,7 +1050,7 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_p2(const __grid_constan
   P2Acc pa{0ll, 0.0};
   const WarpRange R = load_range(A.tm, blockIdx.x * (EM_THREADS / 32) + (threadIdx.x >> 5));
   ring_prefetch(A.tm, W, R);
-  run_phase<2, CH, RING, VBEM, false>(A, W, R, blockIdx.x, gridDim.x, logNorm, bias, pa, NoDeliver{});
+  run_phase<2, CH, RING, VBEM, false>(A, W, R, blockIdx.x, gridDim.x, logNorm, bias, pa, Nothing{}, NoDeliver{});
   p2_finish(A, scratch, pa, par);
 }
 template <int CH, int RING, int MINB, bool VBEM>
@@ -961,7 +1061,7 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_p2_partial(const __grid
   P2Acc pa{0ll, 0.0};
   const WarpRange R = load_range(A.tm, blockIdx.x * (EM_THREADS / 32) + (threadIdx.x >> 5));
   ring_prefetch(A.tm, W, R);
-  run_phase<3, CH, RING, VBEM, false>(A, W, R, blockIdx.x, gridDim.x, 0.0, 0.0, pa, DeliverLocal{A.part_out});
+  run_phase<3, CH, RING, VBEM, false>(A, W, R, blockIdx.x, gridDim.x, 0.0, 0.0, pa, Nothing{}, DeliverLocal{A.part_out});
 }
 
 }  // namespace sb

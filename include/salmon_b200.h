@@ -456,6 +456,11 @@ typedef struct sb_quant_opts {
   uint32_t shard_index, shard_count;   /* rank / number of ranks of a multi-GPU run (one process per GPU); 0 / 1 on one GPU */
   uint64_t seed;
   const void* nccl_uid;      /* shard_count > 1: the 128 bytes of rank 0's sb_nccl_unique_id(), the same on every rank */
+  /* SAM output (one GPU only; NULL / 0 = off): */
+  const char* write_mappings;     /* --writeMappings[=FILE]: path of the SAM file, "-" = standard output */
+  int32_t write_qualities;        /* --writeQualities: QUAL from the read files instead of '*' */
+  int32_t write_unmapped_names;   /* --writeUnmappedNames: out_dir/aux_info/unmapped_names.txt */
+  const char* cmdline;            /* the @PG CL: field of the SAM header (may be NULL) */
 } sb_quant_opts;
 typedef struct sb_quant_summary {
   uint64_t n_observed, n_mapped, n_too_short, n_trimmed_mates, n_classes, n_batches;
@@ -516,6 +521,59 @@ int sb_map_set_option(sb_map_ctx* ctx, const char* key, int64_t value);
  * has shown a strand yet. */
 int sb_map_lib_counts(const sb_map_ctx* ctx, uint64_t out4[4]);
 int sb_detect_lib_type(int paired, const uint64_t counts4[4]);
+
+/* ---- SAM output of the mapping path (`salmon quant --writeMappings`; format rules: DESIGN.md "SAM output") -------
+ * A sink writes the header (@HD, one @SQ per indexed reference with its indexed length, @PG) when it opens.  Attached
+ * to a mapping context, every sb_map_batch_sam call also formats the batch's alignments on the GPU (a sizing kernel, a
+ * scan, a writing kernel over windows of whole fragments that fit a fixed device buffer) and hands the text to the
+ * sink's writer thread, which writes it in batch order.  sam_path "-" = standard output; either path may be NULL
+ * (unmapped_path: the `<name> <type>` lines of --writeUnmappedNames). */
+typedef struct sb_sam sb_sam;
+#define SB_SAM_QUALITIES 1u   /* QUAL from the reads' quality lines (sb_map_batch_sam then needs them) */
+sb_sam* sb_sam_open(const char* sam_path, const char* unmapped_path, const sb_index* ix, const char* cmdline, uint32_t flags);
+/* waits for the writer, closes the files; < 0 when a write failed */
+int sb_sam_close(sb_sam* sam);
+/* unmapped-names lines the host writes itself (pairs too short to map), appended in call order */
+int sb_sam_write_unmapped(sb_sam* sam, const char* text, size_t len);
+typedef struct sb_sam_stats {
+  uint64_t records, sam_bytes, unmapped_lines, batches, windows;
+  double format_ms;           /* device time of the format kernels (CUDA events), all batches */
+  double copy_ms;             /* host wall time of the windows' device->host copies */
+  double slot_wait_ms;        /* host wall time the mapping thread waited for a page-locked buffer the writer held */
+  double write_ms;            /* writer thread's wall time in fwrite */
+} sb_sam_stats;
+int sb_sam_get_stats(const sb_sam* sam, sb_sam_stats* out);
+/* Attach a sink to a context (NULL detaches).  Without a sink sb_map_batch does exactly what it did before: no side
+ * output, no extra kernel.  The device buffer of one window is "sam_window_bytes" (sb_map_set_option, 256 MiB). */
+int sb_map_attach_sam(sb_map_ctx* ctx, sb_sam* sam);
+/* sb_map_batch + SAM records of the batch.  names: the reads' names (mate 1), concatenated, read i at
+ * names[name_off[i] .. name_off[i+1]); qual_left / qual_right: n_pairs x read_len quality characters (only with
+ * SB_SAM_QUALITIES; NULL otherwise). */
+int sb_map_batch_sam(sb_map_ctx* ctx, const uint8_t* left, const uint8_t* right, uint32_t n_pairs, uint32_t read_len,
+                     const char* names, const uint64_t* name_off, const uint8_t* qual_left, const uint8_t* qual_right,
+                     sb_map_batch_stats* stats);
+
+/* Reads with their names (and optionally qualities): sb_reads_next that also returns, in *meta, the names of the
+ * delivered records of the first mate file (up to the first white space, a trailing "/1" or "/2" removed) and, with
+ * want_quals, both mates' quality lines laid out like the bases (stride bytes per read; FASTA records give 'I').
+ * The arrays belong to the reader and stay valid until its next call. */
+typedef struct sb_read_meta {
+  const char* names;
+  const uint64_t* name_off;        /* [n+1] */
+  const uint8_t* qual_left;        /* NULL unless want_quals */
+  const uint8_t* qual_right;
+} sb_read_meta;
+int64_t sb_reads_next_meta(sb_reads* r, uint32_t max_pairs, uint32_t stride, uint8_t* left, uint8_t* right,
+                           uint32_t* len_left, uint32_t* len_right, int want_quals, sb_read_meta* meta);
+/* sb_reads_bucketed whose callback also receives the rows' names and qualities (trimmed like the bases, read_len per
+ * row).  too_short: called once on the calling thread at the end with the names of the pairs dropped as too short,
+ * one per line (may be NULL). */
+typedef int (*sb_batch_meta_cb)(void* user, const uint8_t* left, const uint8_t* right, uint32_t n_pairs, uint32_t read_len,
+                                const sb_read_meta* meta);
+typedef void (*sb_names_cb)(void* user, const char* names, size_t len);
+int sb_reads_bucketed_meta(sb_reads* rd, uint32_t min_len, uint32_t batch, uint32_t max_read_len, uint32_t threads,
+                           uint32_t shard_index, uint32_t shard_count, int want_quals, sb_batch_meta_cb cb,
+                           sb_names_cb too_short, void* user, sb_bucket_stats* stats);
 
 /* Debug: per-warp phase timestamps (ns) of one iteration of the last persistent run:
  * out[n_warps*16] = {P1 start, P1 end, barrier1 end, P2 start, P2 end, reduce end, barrier2 end, P2 home stream end,

@@ -136,7 +136,19 @@ class sb_quant_opts(C.Structure):
     _fields_ = [("device", C.c_int32), ("batch", C.c_uint32), ("max_read_len", C.c_uint32), ("threads", C.c_uint32),
                 ("dump_eq", C.c_int32), ("dump_eq_weights", C.c_int32), ("num_bootstraps", C.c_uint32),
                 ("num_gibbs", C.c_uint32), ("thinning", C.c_uint32), ("no_gamma_draw", C.c_int32),
-                ("shard_index", C.c_uint32), ("shard_count", C.c_uint32), ("seed", C.c_uint64), ("nccl_uid", C.c_void_p)]
+                ("shard_index", C.c_uint32), ("shard_count", C.c_uint32), ("seed", C.c_uint64), ("nccl_uid", C.c_void_p),
+                ("write_mappings", C.c_char_p), ("write_qualities", C.c_int32), ("write_unmapped_names", C.c_int32),
+                ("cmdline", C.c_char_p)]
+
+
+class sb_read_meta(C.Structure):
+    _fields_ = [("names", C.c_void_p), ("name_off", C.c_void_p), ("qual_left", C.c_void_p), ("qual_right", C.c_void_p)]
+
+
+class sb_sam_stats(C.Structure):
+    _fields_ = [("records", C.c_uint64), ("sam_bytes", C.c_uint64), ("unmapped_lines", C.c_uint64),
+                ("batches", C.c_uint64), ("windows", C.c_uint64), ("format_ms", C.c_double), ("copy_ms", C.c_double),
+                ("slot_wait_ms", C.c_double), ("write_ms", C.c_double)]
 
 
 class sb_quant_summary(C.Structure):
@@ -231,6 +243,15 @@ SYMBOLS = {
     "sb_map_partial_get": (C.c_int, [_P, C.POINTER(sb_map_partial)]),
     "sb_map_project_global": (C.c_int, [_P, C.POINTER(sb_map_partial), C.c_uint32, _P, C.POINTER(sb_map_result)]),
     "sb_map_last_alignments": (C.c_int, [_P, C.c_uint32] + [_P] * 10),
+    "sb_sam_open": (_P, [C.c_char_p, C.c_char_p, _P, C.c_char_p, C.c_uint32]),
+    "sb_sam_close": (C.c_int, [_P]),
+    "sb_sam_write_unmapped": (C.c_int, [_P, C.c_char_p, C.c_size_t]),
+    "sb_sam_get_stats": (C.c_int, [_P, C.POINTER(sb_sam_stats)]),
+    "sb_map_attach_sam": (C.c_int, [_P, _P]),
+    "sb_map_batch_sam": (C.c_int, [_P, _P, _P, C.c_uint32, C.c_uint32, _P, _P, _P, _P, C.POINTER(sb_map_batch_stats)]),
+    "sb_reads_next_meta": (C.c_int64, [_P, C.c_uint32, C.c_uint32, _P, _P, _P, _P, C.c_int, C.POINTER(sb_read_meta)]),
+    "sb_reads_bucketed_meta": (C.c_int, [_P, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                         C.c_int, _P, _P, _P, _P]),
     "sb_host_register": (C.c_int, [_P, C.c_size_t]),
     "sb_host_unregister": (C.c_int, [_P]),
 }
@@ -654,6 +675,30 @@ class MapContext:
         self.last_n = n
         return st
 
+    def attach_sam(self, sam):
+        """sb_map_attach_sam: a SamSink (None detaches)"""
+        _check(self.lib.sb_map_attach_sam(self.h, sam.h if sam is not None else None), "sb_map_attach_sam")
+
+    def map_batch_sam(self, left, right, names, quals=None) -> sb_map_batch_stats:
+        """sb_map_batch_sam: the batch, plus its SAM records for the attached sink.  names: list of str / bytes (one
+        per read); quals: (qual_left[n, L], qual_right[n, L] | None) as uint8 arrays when the sink writes qualities."""
+        left = np.ascontiguousarray(left, dtype=np.uint8)
+        n, L = left.shape
+        rp = None
+        if right is not None:
+            right = np.ascontiguousarray(right, dtype=np.uint8)
+            rp = right.ctypes.data
+        blob, off = pack_names(names)
+        q = [None, None]
+        if quals is not None:
+            q = [np.ascontiguousarray(x, dtype=np.uint8) if x is not None else None for x in quals]
+        st = sb_map_batch_stats()
+        _check(self.lib.sb_map_batch_sam(self.h, left.ctypes.data, rp, n, L, blob.ctypes.data, off.ctypes.data,
+                                         q[0].ctypes.data if q[0] is not None else None,
+                                         q[1].ctypes.data if q[1] is not None else None, C.byref(st)), "sb_map_batch_sam")
+        self.last_n = n
+        return st
+
     def reset(self):
         _check(self.lib.sb_map_reset(self.h), "sb_map_reset")
 
@@ -743,6 +788,57 @@ class MapContext:
             pass
 
 
+# ------------------------------------------------------------------------------ SAM output
+def pack_names(names):
+    """names -> (concatenated bytes as uint8[], offsets uint64[n+1]), the layout sb_map_batch_sam takes"""
+    bs = [x.encode() if isinstance(x, str) else bytes(x) for x in names]
+    off = np.zeros(len(bs) + 1, dtype=np.uint64)
+    off[1:] = np.cumsum([len(x) for x in bs], dtype=np.uint64)
+    blob = np.frombuffer(b"".join(bs) + b"\0", dtype=np.uint8).copy()
+    return blob, off
+
+
+class SamSink:
+    """sb_sam: SAM output (`--writeMappings`) and / or aux_info/unmapped_names.txt lines, written by a thread of its own."""
+
+    def __init__(self, index: Index, sam_path=None, unmapped_path=None, cmdline="", qualities=False):
+        self.lib = load()
+        self.h = self.lib.sb_sam_open(os.fsencode(sam_path) if sam_path else None,
+                                      os.fsencode(unmapped_path) if unmapped_path else None, index.h,
+                                      cmdline.encode(), 1 if qualities else 0)
+        if not self.h:
+            raise SalmonB200Error("sb_sam_open failed: " + self.lib.sb_last_error().decode())
+
+    def write_unmapped(self, text: bytes):
+        _check(self.lib.sb_sam_write_unmapped(self.h, text, len(text)), "sb_sam_write_unmapped")
+
+    def stats(self) -> dict:
+        st = sb_sam_stats()
+        _check(self.lib.sb_sam_get_stats(self.h, C.byref(st)), "sb_sam_get_stats")
+        return {k: getattr(st, k) for k, _ in sb_sam_stats._fields_}
+
+    def close(self):
+        if self.h:
+            h, self.h = self.h, None
+            _check(self.lib.sb_sam_close(h), "sb_sam_close")
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _meta_arrays(m, n, shape, paired):
+    """sb_read_meta of n reads -> (names: list of bytes, qual_left | None, qual_right | None)"""
+    off = _view(m.name_off, n + 1, np.uint64)
+    blob = C.string_at(m.names, int(off[-1])) if n and off[-1] else b""
+    names = [blob[int(off[i]):int(off[i + 1])] for i in range(n)]
+    ql = np.ctypeslib.as_array(C.cast(m.qual_left, C.POINTER(C.c_uint8)), shape=shape) if m.qual_left else None
+    qr = np.ctypeslib.as_array(C.cast(m.qual_right, C.POINTER(C.c_uint8)), shape=shape) if (paired and m.qual_right) else None
+    return names, ql, qr
+
+
 # ------------------------------------------------------------------------------ output seam
 def _names(names):
     arr = (C.c_char_p * len(names))(*[n.encode() for n in names])
@@ -815,6 +911,53 @@ class ReadFiles:
                                    lr.ctypes.data if self.paired else None)
         _check(n, "sb_reads_next")
         return n, left[:n], (right[:n] if self.paired else None), ll[:n], (lr[:n] if self.paired else None)
+
+    def next_batch_meta(self, max_pairs, stride, quals=False):
+        """sb_reads_next_meta -> (n, left, right | None, len_left, len_right | None, names (bytes), qual_left | None,
+        qual_right | None); the quality arrays are [n, stride] copies."""
+        left = np.empty((max_pairs, stride), np.uint8)
+        right = np.empty((max_pairs, stride), np.uint8) if self.paired else None
+        ll = np.empty(max_pairs, np.uint32)
+        lr = np.empty(max_pairs, np.uint32) if self.paired else None
+        m = sb_read_meta()
+        n = self.lib.sb_reads_next_meta(self.h, max_pairs, stride, left.ctypes.data,
+                                        right.ctypes.data if self.paired else None, ll.ctypes.data,
+                                        lr.ctypes.data if self.paired else None, int(quals), C.byref(m))
+        _check(n, "sb_reads_next_meta")
+        names, ql, qr = _meta_arrays(m, n, (n, stride), self.paired)
+        return (n, left[:n], (right[:n] if self.paired else None), ll[:n], (lr[:n] if self.paired else None), names,
+                None if ql is None else ql.copy(), None if qr is None else qr.copy())
+
+    def bucketed_meta(self, fn, min_len=31, batch=65536, max_read_len=256, threads=4, shard_index=0, shard_count=1,
+                      quals=False):
+        """sb_reads_bucketed_meta: fn(left[n, L], right | None, L, names (list of bytes), qual_left | None, qual_right |
+        None) per batch (views of the library's buffers).  -> (stats dict, names of the pairs dropped as too short)."""
+        CB = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(sb_read_meta))
+        NCB = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_size_t)
+        raised, dropped = [], []
+
+        def cb(user, lp, rp, n, L, mp):
+            try:
+                left = np.ctypeslib.as_array(C.cast(lp, C.POINTER(C.c_uint8)), shape=(n, L))
+                right = np.ctypeslib.as_array(C.cast(rp, C.POINTER(C.c_uint8)), shape=(n, L)) if rp else None
+                names, ql, qr = _meta_arrays(mp.contents, n, (n, L), rp is not None)
+                r = fn(left, right, L, names, ql, qr)
+                return int(r) if r else 0
+            except Exception as e:  # noqa: BLE001  (an exception must not unwind through the C frames)
+                raised.append(e)
+                return -1
+
+        def ncb(user, p, n):
+            dropped.extend(C.string_at(p, n).splitlines())
+        cbo, ncbo = CB(cb), NCB(ncb)
+        st = (C.c_uint64 * 6)()
+        rc = self.lib.sb_reads_bucketed_meta(self.h, min_len, batch, max_read_len, threads, shard_index, shard_count,
+                                             int(quals), C.cast(cbo, C.c_void_p), C.cast(ncbo, C.c_void_p), None, st)
+        if raised:
+            raise raised[0]
+        _check(rc, "sb_reads_bucketed_meta")
+        return ({"n_observed": st[0], "n_delivered": st[1], "n_too_short": st[2], "n_trimmed_mates": st[3],
+                 "n_batches": st[4], "n_read_lengths": st[5] & 0xffffffff}, dropped)
 
     def peek(self, max_pairs):
         """-> (n available up to max_pairs, their common read length or 0)"""

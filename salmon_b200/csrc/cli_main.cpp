@@ -74,7 +74,7 @@ int usage() {
           "sb_salmon (salmon-b200 %d): H100-native hot path of salmon\n"
           "  sb_salmon index -t transcripts.fa[.gz] -i index_dir [-k 31] [--gencode] [-d decoys.txt] [--keepDuplicates] [--no-clip]\n"
           "  sb_salmon quant -i index_dir -l IU|ISF|ISR -1 r1.fq[.gz] ... -2 r2.fq[.gz] ... | -l U|SF|SR -r reads.fq[.gz] ...  -o out_dir [--gpus N]\n"
-          "                  [-p threads] [--dumpEq] [--dumpEqWeights]\n"
+          "                  [-p threads] [--dumpEq] [--dumpEqWeights] [--writeMappings[=FILE] | -z] [--writeQualities] [--writeUnmappedNames]\n"
           "                  [--numBootstraps N | --numGibbsSamples N] [--thinningFactor 16] [--noGammaDraw] [--useEM] [--vbPrior 0.01]\n"
           "                  [--perNucleotidePrior] [--maxReadOcc 200] [--maxOccsPerHit 1000] [--minScoreFraction 0.65] [--consensusSlack 0.35]\n"
           "                  [--preMergeChainSubThresh 0.75] [--postMergeChainSubThresh 0.9] [--orphanChainSubThresh 0.95] [--allowDovetail]\n"
@@ -213,7 +213,7 @@ int cmd_quant(Args& a) {
   double d = 0;
   bool vb_prior_given = false, pre_merge_given = false, threads_given = false;
   int n_gpus = 1, my_rank = -1;
-  std::string run_tag;
+  std::string run_tag, sam_path;
   while (a.more()) {
     const std::string o = a.next();
     if (o == "-i" || o == "--index") { if (!a.value(dir)) return usage(); }
@@ -269,13 +269,27 @@ int cmd_quant(Args& a) {
     else if (o == "--maxReadLen") { if (!num(d)) return usage(); qo.max_read_len = (uint32_t)d; }
     else if (o == "--seed") { if (!num(d)) return usage(); qo.seed = (uint64_t)d; mp.seed = (uint64_t)d; }
     else if (o == "--validateMappings" || o == "--softclipOverhangs" || o == "-q" || o == "--quiet") { /* default behaviour / no-op */ }
-    else if (o == "--seqBias" || o == "--gcBias" || o == "--posBias" || o == "--writeMappings" || o == "-z" || o == "-a" ||
+    else if (o == "--writeMappings" || o == "-z") sam_path = "-";   // (SAM on standard output)
+    else if (o.rfind("--writeMappings=", 0) == 0) sam_path = o.substr(16);
+    else if (o == "--writeQualities") qo.write_qualities = 1;
+    else if (o == "--writeUnmappedNames") qo.write_unmapped_names = 1;
+    else if (o == "--seqBias" || o == "--gcBias" || o == "--posBias" || o == "-a" ||
              o == "--alignments" || o == "--recoverOrphans" || o == "-g" || o == "--geneMap" || o == "--sketchMode") {
       fprintf(stderr, "sb_salmon quant: %s is outside the hot path this build replaces (DESIGN.md, out of scope)\n", o.c_str());
       return 1;
     } else { fprintf(stderr, "sb_salmon quant: unknown option %s\n", o.c_str()); return usage(); }
   }
   if (out.empty()) return usage();
+  if (n_gpus > 1 && (!sam_path.empty() || qo.write_unmapped_names)) {
+    fprintf(stderr, "sb_salmon quant: --writeMappings / --writeUnmappedNames are written by a one-GPU run only: a read-sharded "
+                    "--gpus %d run cannot write them\n", n_gpus);
+    return 1;
+  }
+  if (sam_path.empty() && qo.write_qualities) { fprintf(stderr, "sb_salmon quant: --writeQualities needs --writeMappings\n"); return 1; }
+  std::string cmdline = "sb_salmon quant";
+  for (const std::string& arg : a.all) cmdline += " " + arg;
+  if (!sam_path.empty()) qo.write_mappings = sam_path.c_str();
+  qo.cmdline = cmdline.c_str();
   if (!threads_given) {   // host threads for the reader (inflate, scan, translate): half the hardware threads, 32 at most
     const unsigned hw = std::thread::hardware_concurrency();
     qo.threads = std::max(2u, std::min(32u, hw / 2 / (unsigned)std::max(1, n_gpus)));   // (per rank)

@@ -592,7 +592,40 @@ struct sb_reads {
   uint32_t max_len_seen = 0;
   bool failed = false;
   double t_wait_blocks = 0, t_translate = 0;
+  // sb_reads_next_meta: names / qualities of the last delivery
+  std::vector<const char*> name_src;
+  std::vector<uint32_t> name_len;
+  std::string names;
+  std::vector<uint64_t> name_off;
+  std::vector<uint8_t> qual[2];
 };
+
+namespace {
+// The header line of the record whose sequence line starts at buf + seq_off: it ends just before the sequence line
+// and starts at the block's start or after a newline.
+inline const char* record_header(const char* buf, uint32_t seq_off) {
+  int64_t i = (int64_t)seq_off - 2;   // (buf[seq_off - 1] is the header's newline)
+  while (i >= 0 && buf[i] != '\n') --i;
+  return buf + i + 1;
+}
+// QNAME: the header after '@' / '>' up to the first white space, a trailing "/1" or "/2" removed
+inline uint32_t read_name(const char* hdr, const char** start) {
+  const char* p = hdr + 1;
+  uint32_t n = 0;
+  while (p[n] != '\n' && p[n] != '\r' && p[n] != ' ' && p[n] != '\t') ++n;
+  if (n >= 2 && p[n - 2] == '/' && (p[n - 1] == '1' || p[n - 1] == '2')) n -= 2;
+  *start = p;
+  return n;
+}
+// the quality line of a FASTQ record (sequence line at seq_off, len characters before its line end)
+inline const char* record_quality(const char* buf, uint32_t seq_off, uint32_t len) {
+  const char* p = buf + seq_off + len;
+  if (*p == '\r') ++p;
+  ++p;                                         // '\n'; now at the '+' line
+  while (*p != '\n') ++p;
+  return p + 1;
+}
+}  // namespace
 
 extern "C" sb_reads* sb_reads_open(const char* const* files1, const char* const* files2, uint32_t n_files,
                                    uint32_t n_threads) {
@@ -638,8 +671,8 @@ extern "C" void sb_reads_close(sb_reads* r) {
   delete r;
 }
 
-extern "C" int64_t sb_reads_next(sb_reads* r, uint32_t max_pairs, uint32_t stride, uint8_t* left, uint8_t* right,
-                                 uint32_t* len_left, uint32_t* len_right) {
+static int64_t reads_next(sb_reads* r, uint32_t max_pairs, uint32_t stride, uint8_t* left, uint8_t* right,
+                          uint32_t* len_left, uint32_t* len_right, bool want_names, bool want_quals) {
   if (!r || !left || !len_left || !stride || (r->n_streams == 2 && (!right || !len_right))) {
     sb::set_error("sb_reads_next: null argument"); return SB_ERR_INVALID;
   }
@@ -673,6 +706,9 @@ extern "C" int64_t sb_reads_next(sb_reads* r, uint32_t max_pairs, uint32_t strid
   const double tw1 = wall();
   r->t_wait_blocks += tw1 - tw0;
   const int nt = (int)std::max<size_t>(1, std::min<size_t>(r->n_threads, tasks.size()));
+  if (want_names) { r->name_src.resize(filled[0]); r->name_len.resize(filled[0]); }
+  if (want_quals)
+    for (int m = 0; m < r->n_streams; ++m) r->qual[m].resize((size_t)filled[m] * stride);
 #pragma omp parallel for schedule(dynamic, 1) num_threads(nt) reduction(max : maxlen)
   for (long ti = 0; ti < (long)tasks.size(); ++ti) {
     const Task& t = tasks[ti];
@@ -687,7 +723,25 @@ extern "C" int64_t sb_reads_next(sb_reads* r, uint32_t max_pairs, uint32_t strid
       uint8_t* d = out + (t.dst + i) * (size_t)stride;
       translate(src, d, n);
       if (n < stride) memset(d + n, 4, stride - n);
+      if (want_names || want_quals) {
+        const char* hdr = record_header(t.blk->buf, off);
+        if (want_names && t.mate == 0) r->name_len[t.dst + i] = read_name(hdr, &r->name_src[t.dst + i]);
+        if (want_quals) {
+          uint8_t* q = r->qual[t.mate].data() + (t.dst + i) * (size_t)stride;
+          if (hdr[0] == '@') memcpy(q, record_quality(t.blk->buf, off, len), n);
+          else memset(q, 'I', n);
+        }
+      }
     }
+  }
+  if (want_names) {
+    const uint64_t nn = filled[0];
+    r->name_off.resize(nn + 1);
+    r->name_off[0] = 0;
+    for (uint64_t i = 0; i < nn; ++i) r->name_off[i + 1] = r->name_off[i] + r->name_len[i];
+    r->names.resize(r->name_off[nn]);
+#pragma omp parallel for schedule(static) num_threads(nt)
+    for (int64_t i = 0; i < (int64_t)nn; ++i) memcpy(&r->names[r->name_off[i]], r->name_src[i], r->name_len[i]);
   }
   r->t_translate += wall() - tw1;
   for (int m = 0; m < r->n_streams; ++m) consume(r->st[m], filled[m]);
@@ -699,6 +753,23 @@ extern "C" int64_t sb_reads_next(sb_reads* r, uint32_t max_pairs, uint32_t strid
   }
   r->n_delivered += filled[0];
   return (int64_t)filled[0];
+}
+
+extern "C" int64_t sb_reads_next(sb_reads* r, uint32_t max_pairs, uint32_t stride, uint8_t* left, uint8_t* right,
+                                 uint32_t* len_left, uint32_t* len_right) {
+  return reads_next(r, max_pairs, stride, left, right, len_left, len_right, false, false);
+}
+
+extern "C" int64_t sb_reads_next_meta(sb_reads* r, uint32_t max_pairs, uint32_t stride, uint8_t* left, uint8_t* right,
+                                      uint32_t* len_left, uint32_t* len_right, int want_quals, sb_read_meta* meta) {
+  if (!meta) { sb::set_error("sb_reads_next_meta: null argument"); return SB_ERR_INVALID; }
+  const int64_t got = reads_next(r, max_pairs, stride, left, right, len_left, len_right, true, want_quals != 0);
+  if (got < 0) return got;
+  meta->names = r->names.data();
+  meta->name_off = r->name_off.data();
+  meta->qual_left = want_quals ? r->qual[0].data() : nullptr;
+  meta->qual_right = (want_quals && r->n_streams == 2) ? r->qual[1].data() : nullptr;
+  return got;
 }
 
 // Look at the lengths of the next records without delivering them: returns how many records (pairs) the next call can

@@ -21,6 +21,7 @@
 #include "common.cuh"
 #include "map_core.h"
 #include "map_kernels.cuh"
+#include "sam_internal.h"
 
 using namespace sbmap;
 
@@ -547,8 +548,12 @@ __global__ void k_assign_work(uint32_t n, const uint32_t* __restrict__ n_l, cons
   work[r] = w; ids[r] = r;
 }
 
+// SAM: a sink is attached -- also fill the side output (per-mate scores, decoy alignments); `side` holds the chunk's
+// base pointers.  The instance without it is the default path, unchanged.
+template <bool SAM>
 __global__ void k_assign(IndexView ix, Params p, FldView fld, int useAux, int burnedIn, uint32_t n, uint32_t L,
-                         BatchBufs b, OnlineView on, uint32_t chunk_first_read, const uint32_t* __restrict__ order) {
+                         BatchBufs b, OnlineView on, uint32_t chunk_first_read, const uint32_t* __restrict__ order,
+                         SamSide side) {
   const uint32_t T = gridDim.x * blockDim.x;
   const uint32_t tid0 = blockIdx.x * blockDim.x + threadIdx.x;
   const uint32_t cap = p.max_read_occ;
@@ -561,8 +566,19 @@ __global__ void k_assign(IndexView ix, Params p, FldView fld, int useAux, int bu
     o.tid = b.tid + (size_t)r * cap; o.score = b.score + (size_t)r * cap; o.prob = b.prob + (size_t)r * cap;
     o.pos = b.pos + (size_t)r * cap; o.mate_pos = b.mate_pos + (size_t)r * cap; o.flags = b.flags + (size_t)r * cap;
     o.flen = b.flen + (size_t)r * cap; o.label = b.label + (size_t)r * 2 * cap; o.weight = b.weight + (size_t)r * cap;
+    SamSide sd;
+    const SamSide* sdp = nullptr;
+    if (SAM) {
+      sd.n_out = side.n_out + r; sd.decoy = side.decoy + r;
+      sd.score1 = side.score1 + (size_t)r * cap; sd.score2 = side.score2 + (size_t)r * cap;
+      sdp = &sd;
+    }
     const uint32_t nlr = b.n_l[r];
-    if (nlr & 0x80000000u) { *o.n_aln = 0; continue; }
+    if (nlr & 0x80000000u) {
+      *o.n_aln = 0;
+      if (SAM) { *sd.n_out = 0; *sd.decoy = 0; }
+      continue;
+    }
     const uint32_t nl = nlr, nr = b.n_r[r];
     if (nl * nr <= 32u && nl + nr <= 32u) {
       // common case: few joint hits -> per-thread scratch in local memory (interleaved across threads, L1-cached)
@@ -577,13 +593,13 @@ __global__ void k_assign(IndexView ix, Params p, FldView fld, int useAux, int bu
       for (uint32_t a = 0; a < nl; ++a) { lcl[a] = gl[a]; sl[a] = b.score_l[(size_t)r * MAXCAND + a]; }
       for (uint32_t a = 0; a < nr; ++a) { rcl[a] = gr[a]; sr[a] = b.score_r[(size_t)r * MAXCAND + a]; }
       assign_read(ix, p, fld, useAux != 0, burnedIn != 0, lcl, nl, rcl, nr, sl, sr, L, sc, pi, pt, b1, b2, b3, jh, o, ctr,
-                  &on, chunk_first_read + r, lp);
+                  &on, chunk_first_read + r, lp, sdp);
     } else {
       const size_t so = (size_t)tid0 * cap;
       assign_read(ix, p, fld, useAux != 0, burnedIn != 0, b.cand_l + (size_t)r * MAXCAND, nl,
                   b.cand_r + (size_t)r * MAXCAND, nr, b.score_l + (size_t)r * MAXCAND,
                   b.score_r + (size_t)r * MAXCAND, L, b.sc + so, b.perm_idx + so, b.perm_tid + so, b.bs_tid + so,
-                  b.bs_score + so, b.bs_idx + so, b.jh + so, o, ctr, &on, chunk_first_read + r, b.lp + so);
+                  b.bs_score + so, b.bs_idx + so, b.jh + so, o, ctr, &on, chunk_first_read + r, b.lp + so, sdp);
     }
   }
   add_counters(b.ctr, ctr);
@@ -1018,6 +1034,10 @@ struct sb_map_ctx {
   std::vector<uint64_t> h_off, h_counts;
   std::vector<uint32_t> h_tids, h_ntx, h_bins;
   std::vector<double> h_w;
+  // SAM output (sb_map_attach_sam): the sink, the formatter's device buffers, the size of one output window
+  sb_sam* sam = nullptr;
+  SamDev* samd = nullptr;
+  uint64_t sam_window = 256ull << 20;
 };
 
 template <typename T>
@@ -1261,6 +1281,7 @@ extern "C" void sb_map_destroy(sb_map_ctx* c) {
                   c->fin.head, c->fin.head_scan, c->fin.start, c->fin.proj, c->fin.eff, c->fin.bound, c->fin.tmp};
   for (void* p : ptrs) cudaFree(p);
   cudaFree(c->d_dummy_mate);
+  sam_dev_destroy(c->samd);
   cudaFree(c->alt_n_l); cudaFree(c->alt_n_r); cudaFree(c->alt_cand_l); cudaFree(c->alt_cand_r); cudaFree(c->alt_score_l); cudaFree(c->alt_score_r);
   for (int s = 0; s < 2; ++s) { if (c->ev_dp[s]) cudaEventDestroy(c->ev_dp[s]); if (c->ev_asg[s]) cudaEventDestroy(c->ev_asg[s]); }
   if (c->assign_stream) cudaStreamDestroy(c->assign_stream);
@@ -1287,6 +1308,11 @@ extern "C" int sb_map_set_option(sb_map_ctx* c, const char* key, int64_t value) 
     return SB_OK;
   }
   if (!strcmp(key, "overlap_assign")) { c->overlap_assign = value ? 1 : 0; return SB_OK; }
+  if (!strcmp(key, "sam_window_bytes")) {
+    if (value < 1) { sb::set_error("sam_window_bytes must be positive"); return SB_ERR_INVALID; }
+    c->sam_window = (uint64_t)value;
+    return SB_OK;
+  }
   if (!strcmp(key, "lib_type")) {   // the expected format of the batches that follow, inside the context's family
     if (value < 0 || value > 5 || (value >= 3) != (c->p.lib_type >= 3)) {
       sb::set_error("lib_type %lld does not fit this context (paired-end: 0..2, single-end: 3..5)", (long long)value);
@@ -1371,8 +1397,9 @@ static int aggregate(sb_map_ctx* c, Records R, EqStore& out) {
   return SB_OK;
 }
 
-extern "C" int sb_map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, uint32_t n, uint32_t L,
-                            sb_map_batch_stats* stats) {
+// sam: the batch's side output for the attached SAM sink is filled (sb_map_batch_sam formats it afterwards)
+static int map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, uint32_t n, uint32_t L,
+                     sb_map_batch_stats* stats, bool sam) {
   if (!c || (n && !left)) { sb::set_error("null argument"); return SB_ERR_INVALID; }
   const bool single_end = c->p.lib_type >= 3;
   if (n && single_end != (right == nullptr)) {
@@ -1497,7 +1524,13 @@ extern "C" int sb_map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* r
       size_t tb = c->agg.tmp_bytes;
       SB_CUDA(cub::DeviceRadixSort::SortPairs(c->agg.tmp, tb, c->d_work, c->d_work2, c->d_ids, c->d_order, (int)cn, 0, 8, as));
     }
-    k_assign<<<T / 128, 128, 0, as>>>(ix, p, c->fld, useAux, burnedIn, cn, L, bc, onv, c0, c->d_order);
+    if (sam) {
+      SamSide sd = sam_dev_side(c->samd);
+      sd.n_out += c0; sd.decoy += c0; sd.score1 += (size_t)c0 * cap; sd.score2 += (size_t)c0 * cap;
+      k_assign<true><<<T / 128, 128, 0, as>>>(ix, p, c->fld, useAux, burnedIn, cn, L, bc, onv, c0, c->d_order, sd);
+    } else {
+      k_assign<false><<<T / 128, 128, 0, as>>>(ix, p, c->fld, useAux, burnedIn, cn, L, bc, onv, c0, c->d_order, SamSide{});
+    }
     c->launches += 3;
     if (ovl) SB_CUDA(cudaEventRecord(c->ev_asg[set], as));
     else SB_CUDA(cudaEventRecord(c->ev_free[s], st));
@@ -1568,6 +1601,40 @@ extern "C" int sb_map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* r
       }
   }
   return SB_OK;
+}
+
+extern "C" int sb_map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, uint32_t n, uint32_t L,
+                            sb_map_batch_stats* stats) {
+  return map_batch(c, left, right, n, L, stats, false);
+}
+
+extern "C" int sb_map_attach_sam(sb_map_ctx* c, sb_sam* sam) {
+  if (!c) { sb::set_error("null argument"); return SB_ERR_INVALID; }
+  SB_CUDA(cudaSetDevice(c->device));
+  SB_CUDA(cudaDeviceSynchronize());
+  sam_dev_destroy(c->samd);
+  c->samd = nullptr;
+  c->sam = nullptr;
+  if (!sam) return SB_OK;
+  SamDev* d = nullptr;
+  const int rc = sam_dev_create(&d, sam, c->batch_cap, c->read_len_cap, c->p.max_read_occ);
+  if (rc != SB_OK) { sam_dev_destroy(d); return rc; }
+  c->samd = d;
+  c->sam = sam;
+  return SB_OK;
+}
+
+extern "C" int sb_map_batch_sam(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, uint32_t n, uint32_t L,
+                                const char* names, const uint64_t* name_off, const uint8_t* qual_left,
+                                const uint8_t* qual_right, sb_map_batch_stats* stats) {
+  if (!c || !c->sam) { sb::set_error("sb_map_batch_sam: no SAM sink attached (sb_map_attach_sam)"); return SB_ERR_STATE; }
+  if (n && (!names || !name_off)) { sb::set_error("sb_map_batch_sam: the reads' names are needed"); return SB_ERR_INVALID; }
+  SB_TRY(map_batch(c, left, right, n, L, stats, true));
+  SamBatch sb;
+  sb.n = n; sb.L = L; sb.cap = c->p.max_read_occ; sb.paired = c->p.lib_type < 3 ? 1 : 0; sb.ascii = c->ascii;
+  sb.tid = c->b.tid; sb.pos = c->b.pos; sb.mate_pos = c->b.mate_pos; sb.flags = c->b.flags; sb.flen = c->b.flen;
+  float ms = 0;
+  return sam_dev_format(c->samd, c->stream, sb, left, right, names, name_off, qual_left, qual_right, c->sam_window, &ms);
 }
 
 extern "C" int sb_map_lib_counts(const sb_map_ctx* c, uint64_t out4[4]) {

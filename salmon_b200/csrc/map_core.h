@@ -555,6 +555,22 @@ struct ReadOut {
   double* weight;        // [cap]
 };
 
+// Side output of the SAM writer, per read (one slot; cap entries for the per-alignment arrays).  Only filled when a
+// SAM sink is attached; the default path passes nullptr and computes exactly what it computes without it.
+//   n_out:   alignments written for the fragment: the kept ones (= *n_aln), or -- when the fragment's best hit is a
+//            decoy -- its equally-best decoy alignments, stored in the ReadOut's tid / pos / mate_pos / flags / flen
+//            arrays with *n_aln = 0 (filterAndCollectAlignmentsDecoy, SalmonMappingUtils.hpp:407-470), so they still
+//            add nothing to the classes;
+//   decoy:   1 when those are decoy alignments;
+//   score1 / score2: each written alignment's own DP score of mate 1 / mate 2 (0 for an absent mate), which SAM
+//            writes as AS:i (salmon's score / mateScore, not the pair sum).
+struct SamSide {
+  uint32_t* n_out;
+  uint8_t* decoy;
+  int32_t* score1;
+  int32_t* score2;
+};
+
 // updateRefMappings + filterAndCollectAlignments + auxiliary probabilities + label, for one read.
 // score_l / score_r: DP score per left / right candidate.  perm_* scratch: >= nj entries each.
 SB_HD void assign_read(const IndexView& ix, const Params& p, const FldView& fld, bool useAux, bool burnedIn,
@@ -562,10 +578,11 @@ SB_HD void assign_read(const IndexView& ix, const Params& p, const FldView& fld,
                        const int32_t* score_r, uint32_t L, int32_t* sc, int32_t* perm_idx, int32_t* perm_tid,
                        int32_t* bs_tid, int32_t* bs_score, int32_t* bs_idx, Joint* jh, const ReadOut& o,
                        Counters& ctr, const OnlineView* on = nullptr, uint32_t read_in_batch = 0,
-                       double* lpbuf = nullptr /* >= cap doubles */) {
+                       double* lpbuf = nullptr /* >= cap doubles */, const SamSide* side = nullptr) {
   const double LOG_EPSILON = -24.006680182952184;   // log(0.375e-10), SalmonMath.hpp:44-45 (libm and sbm_det_log agree)
   const uint32_t cap = p.max_read_occ;
   *o.n_aln = 0;
+  if (side) { *side->n_out = 0; *side->decoy = 0; }
   uint32_t nj = 0;
   const uint32_t total = for_each_joint(p, lc, nl, rcd, nr, L, [&](const Joint& j, uint32_t k) {
     if (k < cap) jh[k] = j;
@@ -600,6 +617,7 @@ SB_HD void assign_read(const IndexView& ix, const Params& p, const FldView& fld,
     perm_idx[nperm] = (int32_t)h; perm_tid[nperm] = (int32_t)jh[h].tid; ++nperm;
   }
   // ---- :283-405
+  const int32_t bestDecoyHit = bestDecoyScore;
   if (bestDecoyScore == INVALID_SCORE) bestDecoyScore = INVALID_SCORE + 1;
   const int32_t decoyThreshold = (int32_t)(p.decoy_threshold * (double)bestDecoyScore);
   const int32_t scoreThreshold = p.hard_filter ? bestScore : decoyThreshold;
@@ -629,10 +647,39 @@ SB_HD void assign_read(const IndexView& ix, const Params& p, const FldView& fld,
     fl |= (uint8_t)(j.status << 2);
     o.flags[na] = fl;
     o.flen[na] = j.frag_len;
+    if (side) {
+      side->score1[na] = j.li >= 0 ? score_l[j.li] : 0;
+      side->score2[na] = j.ri >= 0 ? score_r[j.ri] : 0;
+    }
     ++na;
   }
   *o.n_aln = na;
   ctr.kept += na;
+  if (side) {
+    *side->n_out = na;
+    // only decoy mappings (MappingScoreInfo::haveOnlyDecoyMappings, SalmonMappingUtils.hpp:115-122): the equally-best
+    // decoy hits, in joint-hit order, are written to the SAM output and nowhere else
+    if (na == 0 && bestDecoyHit != INVALID_SCORE && bestScore < (int32_t)(p.decoy_threshold * (double)bestDecoyHit)) {
+      uint32_t nd = 0;
+      for (uint32_t h = 0; h < nj && nd < cap; ++h) {
+        const Joint& j = jh[h];
+        if ((int32_t)j.tid < p.first_decoy || sc[h] != bestDecoyHit) continue;
+        const Cand& first = (j.status == 2) ? rcd[j.ri] : lc[j.li];
+        o.tid[nd] = j.tid;
+        o.pos[nd] = first.diag_c;
+        o.mate_pos[nd] = (j.status == 0) ? rcd[j.ri].diag_c : 0;
+        uint8_t fl = (uint8_t)(((first.ori_cov >> 31) == 0) ? 1 : 0);
+        if (j.status == 0 && (rcd[j.ri].ori_cov >> 31) == 0) fl |= 2;
+        o.flags[nd] = (uint8_t)(fl | (j.status << 2));
+        o.flen[nd] = j.frag_len;
+        side->score1[nd] = j.li >= 0 ? score_l[j.li] : 0;
+        side->score2[nd] = j.ri >= 0 ? score_r[j.ri] : 0;
+        ++nd;
+      }
+      *side->n_out = nd;
+      *side->decoy = nd ? 1 : 0;
+    }
+  }
   if (na == 0) return;
   ctr.mapped++;
   {   // observed formats of this fragment (libTypeCountsPerFrag, SalmonQuantify.cpp:765,1000-1002): bit 0 ISF, 1 ISR, 2 SF, 3 SR

@@ -45,6 +45,10 @@ struct HostBuf {   // pinned [cap, L] byte matrix pair
   uint32_t cap = 0, L = 0, n = 0;
   bool busy = false;   // handed to the consumer side
   bool pinned = false;
+  // sb_reads_bucketed_meta: the rows' names (concatenated, name_off[row]) and quality lines ([cap, L] per mate)
+  std::string names;
+  std::vector<uint64_t> name_off;
+  std::vector<uint8_t> qual[2];
   int alloc(uint32_t cap_, uint32_t L_) {
     cap = cap_; L = L_; n = 0;
     const size_t bytes = (size_t)cap * L;
@@ -110,10 +114,12 @@ bool make_dirs(const std::string& path) {
 
 }  // namespace
 
-extern "C" int sb_reads_bucketed(sb_reads* rd, uint32_t min_len, uint32_t batch, uint32_t max_read_len, uint32_t threads,
-                                 uint32_t shard_index, uint32_t shard_count, sb_batch_cb cb, void* user,
-                                 sb_bucket_stats* stats) {
-  if (!rd || !cb) { sb::set_error("sb_reads_bucketed: null argument"); return SB_ERR_INVALID; }
+// meta: the meta variant -- names (and with want_quals qualities) travel with their rows to mcb; too-short pairs' names go
+// to too_short at the end
+static int reads_bucketed(sb_reads* rd, uint32_t min_len, uint32_t batch, uint32_t max_read_len, uint32_t threads,
+                          uint32_t shard_index, uint32_t shard_count, sb_batch_cb cb, bool meta, bool want_quals,
+                          sb_batch_meta_cb mcb, sb_names_cb too_short, void* user, sb_bucket_stats* stats) {
+  if (!rd || !(cb || mcb)) { sb::set_error("sb_reads_bucketed: null argument"); return SB_ERR_INVALID; }
   if (batch < 1) batch = 1;
   if (max_read_len < 1) { sb::set_error("sb_reads_bucketed: max_read_len must be positive"); return SB_ERR_INVALID; }
   if (shard_count == 0 || shard_index >= shard_count) { sb::set_error("bad shard index / count"); return SB_ERR_INVALID; }
@@ -129,10 +135,31 @@ extern "C" int sb_reads_bucketed(sb_reads* rd, uint32_t min_len, uint32_t batch,
     P.jobs.push_back(Job{b});
     P.cv_job.notify_one();
   };
+  std::string dropped_names;             // (meta) pairs too short to map, one name per line
   auto reader = [&]() {
     std::vector<uint8_t> sl, sr;          // staging for batches of mixed lengths (allocated on first use)
     std::vector<uint32_t> ll(batch), lr(batch);
     std::string err;
+    sb_read_meta md{};
+    // (meta) rows [i0, i0 + cnt) of the last delivery (quality rows `src_stride` apart) -> rows [row0, ..) of b
+    auto put_meta = [&](HostBuf* b, uint32_t row0, int64_t i0, int64_t cnt, uint32_t src_stride) {
+      if (row0 == 0) { b->names.clear(); b->name_off.assign(1, 0); }
+      for (int64_t q = 0; q < cnt; ++q) {
+        b->names.append(md.names + md.name_off[i0 + q], md.name_off[i0 + q + 1] - md.name_off[i0 + q]);
+        b->name_off.push_back(b->names.size());
+      }
+      if (!want_quals) return;
+      const uint8_t* src[2] = {md.qual_left, md.qual_right};
+      for (int m = 0; m < (paired ? 2 : 1); ++m) {
+        if (b->qual[m].size() < (size_t)b->cap * b->L) b->qual[m].resize((size_t)b->cap * b->L);
+        for (int64_t q = 0; q < cnt; ++q)
+          memcpy(b->qual[m].data() + (size_t)(row0 + q) * b->L, src[m] + (size_t)(i0 + q) * src_stride, b->L);
+      }
+    };
+    auto next = [&](uint32_t n, uint32_t st, uint8_t* l, uint8_t* r) -> int64_t {
+      return meta ? sb_reads_next_meta(rd, n, st, l, r, ll.data(), lr.data(), want_quals ? 1 : 0, &md)
+                  : sb_reads_next(rd, n, st, l, r, ll.data(), lr.data());
+    };
     // the bucket of length L with room for at least one row; nullptr on error / abort
     auto bucket_for = [&](uint32_t L) -> Bucket* {
       std::unique_ptr<Bucket>& bp = buckets[L];
@@ -169,6 +196,7 @@ extern "C" int sb_reads_bucketed(sb_reads* rd, uint32_t min_len, uint32_t batch,
           memcpy(b->left + (size_t)(bp->cnt + q) * L, sl.data() + (size_t)(i0 + q) * stride, L);
           if (paired) memcpy(b->right + (size_t)(bp->cnt + q) * L, sr.data() + (size_t)(i0 + q) * stride, L);
         }
+        if (meta) put_meta(b, bp->cnt, i0, take, stride);
         i0 += take;
         filled(bp, (uint32_t)take);
       }
@@ -193,16 +221,16 @@ extern "C" int sb_reads_bucketed(sb_reads* rd, uint32_t min_len, uint32_t batch,
           if (!bp) break;
           HostBuf* b = &bp->buf[bp->fill];
           const uint32_t take = (uint32_t)std::min<int64_t>(left_n, (int64_t)(b->cap - bp->cnt));
-          const int64_t got = sb_reads_next(rd, take, L0, b->left + (size_t)bp->cnt * L0, b->right + (size_t)bp->cnt * L0,
-                                            ll.data(), lr.data());
+          const int64_t got = next(take, L0, b->left + (size_t)bp->cnt * L0, b->right + (size_t)bp->cnt * L0);
           if (got != (int64_t)take) { err = got < 0 ? sb_last_error() : "short read from the parser"; break; }
+          if (meta) put_meta(b, bp->cnt, 0, take, L0);
           left_n -= take;
           filled(bp, take);
         }
         continue;
       }
       if (sl.empty()) { sl.resize((size_t)batch * stride); sr.resize((size_t)batch * stride); }
-      const int64_t got = sb_reads_next(rd, (uint32_t)n, stride, sl.data(), sr.data(), ll.data(), lr.data());
+      const int64_t got = next((uint32_t)n, stride, sl.data(), sr.data());
       if (got != n) { err = got < 0 ? sb_last_error() : "short read from the parser"; break; }
       // runs of equal length go in one piece
       int64_t run0 = 0;
@@ -212,7 +240,11 @@ extern "C" int sb_reads_bucketed(sb_reads* rd, uint32_t min_len, uint32_t batch,
         if (i < n) {
           L = paired ? std::min(ll[i], lr[i]) : ll[i];
           if (paired && ll[i] != lr[i]) ++P.n_trimmed_mates;
-          if (L < min_len || L == 0) { ++P.n_too_short; L = 0; }   // cannot hold a k-mer: observed, never delivered
+          if (L < min_len || L == 0) {   // cannot hold a k-mer: observed, never delivered
+            ++P.n_too_short;
+            L = 0;
+            if (meta) { dropped_names.append(md.names + md.name_off[i], md.name_off[i + 1] - md.name_off[i]); dropped_names += '\n'; }
+          }
         }
         if (i == n || L != runL) {
           if (runL != 0 && i > run0) put_rows(runL, run0, i);
@@ -250,7 +282,13 @@ extern "C" int sb_reads_bucketed(sb_reads* rd, uint32_t min_len, uint32_t batch,
     }
     if (rc == SB_OK) {
       const double tc = now_s();
-      rc = cb(user, j.b->left, paired ? j.b->right : nullptr, j.b->n, j.b->L);
+      if (meta) {
+        sb_read_meta m{j.b->names.data(), j.b->name_off.data(), want_quals ? j.b->qual[0].data() : nullptr,
+                       (want_quals && paired) ? j.b->qual[1].data() : nullptr};
+        rc = mcb(user, j.b->left, paired ? j.b->right : nullptr, j.b->n, j.b->L, &m);
+      } else {
+        rc = cb(user, j.b->left, paired ? j.b->right : nullptr, j.b->n, j.b->L);
+      }
       t_cb += now_s() - tc;
       if (rc != SB_OK) {
         cb_err = sb_last_error();
@@ -281,7 +319,24 @@ extern "C" int sb_reads_bucketed(sb_reads* rd, uint32_t min_len, uint32_t batch,
   }
   if (rc != SB_OK) { sb::set_error("%s", cb_err.c_str()); return rc > 0 ? SB_ERR_STATE : rc; }
   if (!P.err.empty()) { sb::set_error("%s", P.err.c_str()); return SB_ERR_INVALID; }
+  if (meta && too_short && !dropped_names.empty()) too_short(user, dropped_names.data(), dropped_names.size());
   return SB_OK;
+}
+
+extern "C" int sb_reads_bucketed(sb_reads* rd, uint32_t min_len, uint32_t batch, uint32_t max_read_len, uint32_t threads,
+                                 uint32_t shard_index, uint32_t shard_count, sb_batch_cb cb, void* user,
+                                 sb_bucket_stats* stats) {
+  if (!cb) { sb::set_error("sb_reads_bucketed: null argument"); return SB_ERR_INVALID; }
+  return reads_bucketed(rd, min_len, batch, max_read_len, threads, shard_index, shard_count, cb, false, false, nullptr,
+                        nullptr, user, stats);
+}
+
+extern "C" int sb_reads_bucketed_meta(sb_reads* rd, uint32_t min_len, uint32_t batch, uint32_t max_read_len, uint32_t threads,
+                                      uint32_t shard_index, uint32_t shard_count, int want_quals, sb_batch_meta_cb cb,
+                                      sb_names_cb too_short, void* user, sb_bucket_stats* stats) {
+  if (!cb) { sb::set_error("sb_reads_bucketed_meta: null argument"); return SB_ERR_INVALID; }
+  return reads_bucketed(rd, min_len, batch, max_read_len, threads, shard_index, shard_count, nullptr, true, want_quals != 0,
+                        cb, too_short, user, stats);
 }
 
 extern "C" void sb_quant_default_opts(sb_quant_opts* o) {
@@ -500,6 +555,13 @@ extern "C" int sb_quant_files(sb_index* ix, const char* const* mates1, const cha
     return SB_ERR_INVALID;
   }
   if (o.num_bootstraps && o.num_gibbs) { sb::set_error("choose bootstraps or Gibbs samples, not both"); return SB_ERR_INVALID; }
+  const bool sam_out = o.write_mappings || o.write_unmapped_names;
+  if (multi && sam_out) {
+    sb::set_error("--writeMappings / --writeUnmappedNames are written by a one-GPU run only: a read-sharded run (--gpus N) "
+                  "cannot write them");
+    return SB_ERR_INVALID;
+  }
+  if (o.write_unmapped_names && !out_dir) { sb::set_error("--writeUnmappedNames needs an output directory"); return SB_ERR_INVALID; }
   if (multi && (o.num_bootstraps || o.num_gibbs || o.dump_eq || o.dump_eq_weights)) {
     sb::set_error("posterior samples / --dumpEq need the whole class table on one GPU: run them on one GPU, or sample from a dumped table "
                   "with `quant -e` (which splits the samples over the GPUs)");
@@ -535,8 +597,14 @@ extern "C" int sb_quant_files(sb_index* ix, const char* const* mates1, const cha
   const std::string start_time = time_string();
 
   struct Scope {   // everything acquired below, released on every exit path
-    sb_map_ctx* ctx = nullptr; sb_em_ctx* em = nullptr; sb_comm* comm = nullptr; sb_reads* rd = nullptr;
-    ~Scope() { if (rd) sb_reads_close(rd); if (em) sb_em_destroy(em); if (ctx) sb_map_destroy(ctx); if (comm) sb_comm_destroy(comm); }
+    sb_map_ctx* ctx = nullptr; sb_em_ctx* em = nullptr; sb_comm* comm = nullptr; sb_reads* rd = nullptr; sb_sam* sam = nullptr;
+    ~Scope() {
+      if (rd) sb_reads_close(rd);
+      if (em) sb_em_destroy(em);
+      if (ctx) sb_map_destroy(ctx);
+      if (sam) sb_sam_close(sam);
+      if (comm) sb_comm_destroy(comm);
+    }
   } S;
   if (multi) {
     S.comm = sb_comm_create((int)o.shard_index, (int)o.shard_count, o.nccl_uid, o.device);
@@ -545,33 +613,78 @@ extern "C" int sb_quant_files(sb_index* ix, const char* const* mates1, const cha
   S.ctx = sb_map_create(ix, &mp, o.device, o.batch, o.max_read_len);
   if (!S.ctx) return SB_ERR_CUDA;
   if (getenv("SB_READS_PROFILE")) fprintf(stderr, "sb_quant_files: sb_map_create %.3f s\n", now_s() - t0);
+  if (sam_out) {
+    std::string un;
+    if (o.write_unmapped_names) {
+      un = std::string(out_dir) + "/aux_info";
+      if (!make_dirs(un)) { sb::set_error("cannot create %s", un.c_str()); return SB_ERR_INVALID; }
+      un += "/unmapped_names.txt";
+    }
+    S.sam = sb_sam_open(o.write_mappings, o.write_unmapped_names ? un.c_str() : nullptr, ix, o.cmdline,
+                        o.write_qualities ? SB_SAM_QUALITIES : 0u);
+    if (!S.sam) return SB_ERR_INVALID;
+    SB_TRY(sb_map_attach_sam(S.ctx, S.sam));
+  }
   S.rd = sb_reads_open(mates1, mates2, n_files, o.threads);
   if (!S.rd) return SB_ERR_INVALID;
   const double t_setup = now_s();
 
-  struct MapUser { sb_map_ctx* ctx; float device_ms; bool detect; bool paired; int detected; uint64_t at_fragment, seen; } mu{
-      S.ctx, 0.0f, auto_lib, !single_end, -1, 0, 0};
+  struct MapUser {
+    sb_map_ctx* ctx; float device_ms; bool detect; bool paired; int detected; uint64_t at_fragment, seen;
+    // bookkeeping after a mapped batch: device time, library-type detection
+    int after(const sb_map_batch_stats& st, uint32_t n) {
+      device_ms += st.device_ms;
+      seen += n;
+      int rc = SB_OK;
+      if (detect) {
+        uint64_t c4[4];
+        rc = sb_map_lib_counts(ctx, c4);
+        if (rc == SB_OK && (paired ? c4[0] + c4[1] : c4[2] + c4[3]) >= 50000) {   // numSamplesNeeded_, LibraryTypeDetector.hpp:171
+          detected = sb_detect_lib_type(paired ? 1 : 0, c4);
+          at_fragment = seen;
+          detect = false;
+          if (detected >= 0) rc = sb_map_set_option(ctx, "lib_type", detected);
+        }
+      }
+      return rc;
+    }
+  } mu{S.ctx, 0.0f, auto_lib, !single_end, -1, 0, 0};
   sb_batch_cb map_cb = [](void* user, const uint8_t* l, const uint8_t* r, uint32_t n, uint32_t L) -> int {
     MapUser* u = (MapUser*)user;
     sb_map_batch_stats st;
-    int rc = sb_map_batch(u->ctx, l, r, n, L, &st);
-    if (rc != SB_OK) return rc;
-    u->device_ms += st.device_ms;
-    u->seen += n;
-    if (u->detect) {
-      uint64_t c4[4];
-      rc = sb_map_lib_counts(u->ctx, c4);
-      if (rc == SB_OK && (u->paired ? c4[0] + c4[1] : c4[2] + c4[3]) >= 50000) {   // numSamplesNeeded_, LibraryTypeDetector.hpp:171
-        u->detected = sb_detect_lib_type(u->paired ? 1 : 0, c4);
-        u->at_fragment = u->seen;
-        u->detect = false;
-        if (u->detected >= 0) rc = sb_map_set_option(u->ctx, "lib_type", u->detected);
-      }
-    }
-    return rc;
+    const int rc = sb_map_batch(u->ctx, l, r, n, L, &st);
+    return rc != SB_OK ? rc : u->after(st, n);
   };
   sb_bucket_stats bs;
-  int rc = sb_reads_bucketed(S.rd, mp.k, o.batch, o.max_read_len, o.threads, o.shard_index, o.shard_count, map_cb, &mu, &bs);
+  int rc;
+  if (S.sam) {
+    // the same per-batch work, with the rows' names (and qualities) for the SAM records; pairs too short to map are
+    // listed as unmapped by the host
+    struct SamUser { MapUser* mu; sb_sam* sam; int rc; } su{&mu, S.sam, SB_OK};
+    sb_batch_meta_cb sam_cb = [](void* user, const uint8_t* l, const uint8_t* r, uint32_t n, uint32_t L,
+                                 const sb_read_meta* m) -> int {
+      SamUser* u = (SamUser*)user;
+      sb_map_batch_stats st;
+      const int rc = sb_map_batch_sam(u->mu->ctx, l, r, n, L, m->names, m->name_off, m->qual_left, m->qual_right, &st);
+      return rc != SB_OK ? rc : u->mu->after(st, n);
+    };
+    sb_names_cb short_cb = [](void* user, const char* names, size_t len) {
+      SamUser* u = (SamUser*)user;
+      std::string t;
+      for (size_t i = 0, b = 0; i < len; ++i)
+        if (names[i] == '\n') { t.append(names + b, i - b); t += " u\n"; b = i + 1; }
+      if (u->rc == SB_OK) u->rc = sb_sam_write_unmapped(u->sam, t.data(), t.size());
+    };
+    rc = sb_reads_bucketed_meta(S.rd, mp.k, o.batch, o.max_read_len, o.threads, o.shard_index, o.shard_count,
+                                o.write_qualities ? 1 : 0, sam_cb, short_cb, &su, &bs);
+    if (rc == SB_OK) rc = su.rc;
+    if (rc == SB_OK) rc = sb_map_attach_sam(S.ctx, nullptr);
+    const int rc2 = sb_sam_close(S.sam);
+    S.sam = nullptr;
+    if (rc == SB_OK) rc = rc2;
+  } else {
+    rc = sb_reads_bucketed(S.rd, mp.k, o.batch, o.max_read_len, o.threads, o.shard_index, o.shard_count, map_cb, &mu, &bs);
+  }
   sb_reads_close(S.rd);
   S.rd = nullptr;
   if (rc != SB_OK) return rc;

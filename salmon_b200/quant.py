@@ -141,13 +141,15 @@ def _quantify(index, ctx, ep, device, dist, names, out_dir, dump_eq, dump_eq_wei
 
 
 def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=None, device=0, batch=262_144,
-                max_read_len=256, threads=8, dist=None, dump_eq=False, dump_eq_weights=False, num_bootstraps=0, seed=0):
+                max_read_len=256, threads=8, dist=None, dump_eq=False, dump_eq_weights=False, num_bootstraps=0, seed=0,
+                write_mappings=None, write_qualities=False, write_unmapped_names=False, cmdline=""):
     """`salmon quant -i index -l IU -1 mates1 -2 mates2 -o out_dir` for the hot path: FASTQ/FASTA(.gz) files ->
     sb_reads_bucketed -> sb_map_batch -> ... -> quant.sf.  index: an _capi.Index or the path of a saved one.  With
     torch.distributed initialised every rank takes the global batches g with g % world == rank (round-robin sharding
     of the read stream, SURVEY.md 8e), the end-of-mapping statistics are reduced once and the EM all-reduces alpha.
     A pair whose mates differ in length is mapped at the shorter length (documented deviation until the kernels take
-    per-mate lengths)."""
+    per-mate lengths).  write_mappings: path of a SAM file of the mappings (`--writeMappings=FILE`), with the reads'
+    qualities when write_qualities; write_unmapped_names: out_dir/aux_info/unmapped_names.txt.  Both need one GPU."""
     if isinstance(index, (str, bytes, os.PathLike)):
         index = _capi.Index.load(index)
     mp = map_params or map_default_params()
@@ -163,9 +165,35 @@ def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=
     def map_one(left, right, L):
         ctx.map_batch(left, right)       # raises on error (the reader then stops and reports it)
         return 0
-    with _capi.ReadFiles(mates1, mates2, n_threads=threads) as rf:
-        st = rf.bucketed(map_one, min_len=mp.k, batch=batch, max_read_len=max_read_len, threads=threads,
-                         shard_index=rank, shard_count=world)
+    if write_mappings or write_unmapped_names:
+        if world > 1:
+            raise _capi.SalmonB200Error("write_mappings / write_unmapped_names are written by a one-GPU run only: a "
+                                        "read-sharded run cannot write them")
+        un = None
+        if write_unmapped_names:
+            if out_dir is None:
+                raise _capi.SalmonB200Error("write_unmapped_names needs an output directory")
+            os.makedirs(os.path.join(out_dir, "aux_info"), exist_ok=True)
+            un = os.path.join(out_dir, "aux_info", "unmapped_names.txt")
+        sink = _capi.SamSink(index, write_mappings, un, cmdline=cmdline, qualities=write_qualities)
+        try:
+            ctx.attach_sam(sink)
+
+            def map_sam(left, right, L, names, ql, qr):
+                ctx.map_batch_sam(left, right, names, (ql, qr) if write_qualities else None)
+                return 0
+            with _capi.ReadFiles(mates1, mates2, n_threads=threads) as rf:
+                st, dropped = rf.bucketed_meta(map_sam, min_len=mp.k, batch=batch, max_read_len=max_read_len,
+                                               threads=threads, quals=write_qualities)
+            if dropped:
+                sink.write_unmapped(b"".join(nm + b" u\n" for nm in dropped))
+            ctx.attach_sam(None)
+        finally:
+            sink.close()
+    else:
+        with _capi.ReadFiles(mates1, mates2, n_threads=threads) as rf:
+            st = rf.bucketed(map_one, min_len=mp.k, batch=batch, max_read_len=max_read_len, threads=threads,
+                             shard_index=rank, shard_count=world)
     n_observed = int(st["n_observed"])
     return _quantify(index, ctx, ep, device, dist, None, out_dir, dump_eq, dump_eq_weights, num_bootstraps, seed,
                      n_observed=n_observed)

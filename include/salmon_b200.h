@@ -294,7 +294,10 @@ typedef struct sb_map_params {
    * (single-end: sb_map_batch with right == NULL).  Mappings that are not compatible with it are ignored
    * (incompatPrior = 0 -> ignoreIncompat, SalmonQuantify.cpp:1467-1521,2141-2150; rules src/util/SalmonUtils.cpp:138-298) */
   int32_t lib_type;
-  int32_t reserved3;
+  /* --recoverOrphans (0 = off; paired-end, warp kernels only): for a read whose joint hits are orphans only, search each
+   * anchor's transcript within max_frag_len for the missing mate (infix edit distance) and turn the orphans into the
+   * pairs found (rule: DESIGN.md section 11).  Single-end libraries ignore it. */
+  int32_t recover_orphans;
 } sb_map_params;
 /* Only sb_quant_files takes these two: the library type is detected from the first 50 000 fragments that show a
  * strand, as LibraryTypeDetector does (include/salmon/internal/model/LibraryTypeDetector.hpp:34-140): until then every
@@ -318,6 +321,11 @@ typedef struct sb_map_batch_stats {
   uint64_t full_dp;           /* mate alignments that needed the banded DP (the rest: ungapped shortcut) */
   float seed_kernel_ms;       /* device time of the seed/chain kernel launches of this batch (CUDA events) */
   uint32_t seed_kernel_launches;
+  /* orphan rescue (recover_orphans): fragments with at least one rescued pair, mate searches run, anchors whose mate
+   * was found but whose candidate list had no room; device time of the rescue kernels (CUDA events) */
+  uint64_t orphans_rescued, rescue_searches, rescue_no_room;
+  float rescue_kernel_ms;
+  uint32_t reserved2;
 } sb_map_batch_stats;
 
 typedef struct sb_map_result {   /* host CSR owned by the context, valid until destroy / next finish */
@@ -339,6 +347,7 @@ typedef struct sb_map_result {   /* host CSR owned by the context, valid until d
    * SalmonQuantify.cpp:765,1000-1002): [0] ISF (pair, left mate forward), [1] ISR, [2] SF (orphan / single-end read
    * mapped forward), [3] SR; [4..7] reserved */
   uint64_t lib_format_counts[8];
+  uint64_t orphans_rescued, rescue_searches, rescue_no_room;   /* sums of sb_map_batch_stats' fields since create / reset */
 } sb_map_result;
 
 typedef struct sb_map_ctx sb_map_ctx;
@@ -415,6 +424,12 @@ int sb_map_finish(sb_map_ctx* ctx, sb_map_result* out);
  * hist_out[max_frag_len+1] (log FLD histogram), log_eff_out[n_txps],
  * scalars6 = {assigned fragments, fragments seen, timestep, burned in, FLD min, bits of the log total FLD mass}. */
 int sb_map_online_state(sb_map_ctx* ctx, double* mass_out, double* hist_out, double* log_eff_out, uint64_t* scalars6);
+/* Parity tap of the orphan rescue search (DESIGN.md section 11): case i searches pattern pats[pat_off[i]..pat_off[i+1])
+ * (base codes 0..3, 4 = N, 1..256 bases) in window wins[win_off[i]..win_off[i+1]) with edit limit K[i] on `device`,
+ * with the kernel's own search; dist[i] = the smallest infix edit distance and end[i] = the leftmost window position
+ * where an alignment at that distance ends, both -1 when it exceeds K[i] or the window is empty. */
+int sb_rescue_search_tap(int device, uint32_t n, const uint8_t* pats, const uint64_t* pat_off, const uint8_t* wins,
+                         const uint64_t* win_off, const int32_t* K, int32_t* dist, int32_t* end);
 /* Parity tap: the per-read alignments / labels of the last batch (arrays n*cap; label n*2*cap). */
 int sb_map_last_alignments(sb_map_ctx* ctx, uint32_t n, uint32_t* n_aln, uint32_t* tid, int32_t* score,
                            double* prob, int32_t* pos, int32_t* mate_pos, uint8_t* flags, int32_t* flen,
@@ -469,6 +484,7 @@ typedef struct sb_quant_summary {
   float map_device_ms;                             /* sum of sb_map_batch_stats.device_ms */
   float map_setup_ms;                              /* the part of map_seconds before the first read is parsed: sb_map_create
                                                       (workspace allocation, index upload if not resident) + opening the files */
+  uint64_t orphans_rescued, rescue_searches, rescue_no_room;   /* this rank's orphan rescue counters (sb_map_result) */
 } sb_quant_summary;
 void sb_quant_default_opts(sb_quant_opts* o);
 /* mp / ep / o may be NULL (defaults); out_dir may be NULL (no files); alpha_out[n_txps] may be NULL (decoy entries, the

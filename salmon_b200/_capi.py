@@ -82,7 +82,8 @@ class sb_map_params(C.Structure):
         ("num_pre_burnin", C.c_uint64), ("num_burnin", C.c_uint64),
         ("seed", C.c_uint64), ("mini_batch", C.c_uint32), ("reserved2", C.c_uint32),
         ("pre_merge_thresh", C.c_double), ("post_merge_thresh", C.c_double), ("orphan_thresh", C.c_double),
-        ("allow_dovetail", C.c_int32), ("allow_orphans", C.c_int32), ("lib_type", C.c_int32), ("reserved3", C.c_int32),
+        ("allow_dovetail", C.c_int32), ("allow_orphans", C.c_int32), ("lib_type", C.c_int32),
+        ("recover_orphans", C.c_int32),
     ]
 
 
@@ -90,7 +91,9 @@ class sb_map_batch_stats(C.Structure):
     _fields_ = [("n_pairs", C.c_uint32), ("gpu_launches", C.c_uint32)] + \
         [(k, C.c_uint64) for k in ("mapped", "lookups", "postings", "seeds", "candidates", "kept", "label_entries",
                                    "n_batch_classes")] + [("device_ms", C.c_float), ("reserved", C.c_uint32), ("full_dp", C.c_uint64),
-                                                              ("seed_kernel_ms", C.c_float), ("seed_kernel_launches", C.c_uint32)]
+                                                              ("seed_kernel_ms", C.c_float), ("seed_kernel_launches", C.c_uint32)] + \
+        [(k, C.c_uint64) for k in ("orphans_rescued", "rescue_searches", "rescue_no_room")] + \
+        [("rescue_kernel_ms", C.c_float), ("reserved2", C.c_uint32)]
 
     def asdict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
@@ -102,7 +105,8 @@ class sb_map_result(C.Structure):
         [(k, C.c_uint64) for k in ("n_mapped", "lookups", "postings", "seeds", "candidates", "kept", "label_entries")] + \
         [("n_txps", C.c_uint32), ("reserved", C.c_uint32), ("projected_counts", C.POINTER(C.c_double)),
          ("eff_len", C.POINTER(C.c_double)), ("unique_counts", C.POINTER(C.c_uint64)),
-         ("total_counts", C.POINTER(C.c_uint64)), ("lib_format_counts", C.c_uint64 * 8)]
+         ("total_counts", C.POINTER(C.c_uint64)), ("lib_format_counts", C.c_uint64 * 8)] + \
+        [(k, C.c_uint64) for k in ("orphans_rescued", "rescue_searches", "rescue_no_room")]
 
 
 # every symbol include/salmon_b200.h declares: (name, restype, argtypes)
@@ -156,7 +160,8 @@ class sb_quant_summary(C.Structure):
                 ("n_trimmed_mates", C.c_uint64), ("n_classes", C.c_uint64), ("n_batches", C.c_uint64),
                 ("n_read_lengths", C.c_uint32), ("em_iters", C.c_uint32), ("em_converged", C.c_uint32),
                 ("reserved", C.c_uint32), ("map_seconds", C.c_double), ("em_seconds", C.c_double),
-                ("total_seconds", C.c_double), ("map_device_ms", C.c_float), ("map_setup_ms", C.c_float)]
+                ("total_seconds", C.c_double), ("map_device_ms", C.c_float), ("map_setup_ms", C.c_float)] + \
+        [(k, C.c_uint64) for k in ("orphans_rescued", "rescue_searches", "rescue_no_room")]
 
 
 SYMBOLS = {
@@ -243,6 +248,7 @@ SYMBOLS = {
     "sb_map_partial_get": (C.c_int, [_P, C.POINTER(sb_map_partial)]),
     "sb_map_project_global": (C.c_int, [_P, C.POINTER(sb_map_partial), C.c_uint32, _P, C.POINTER(sb_map_result)]),
     "sb_map_last_alignments": (C.c_int, [_P, C.c_uint32] + [_P] * 10),
+    "sb_rescue_search_tap": (C.c_int, [C.c_int, C.c_uint32] + [_P] * 7),
     "sb_sam_open": (_P, [C.c_char_p, C.c_char_p, _P, C.c_char_p, C.c_uint32]),
     "sb_sam_close": (C.c_int, [_P]),
     "sb_sam_write_unmapped": (C.c_int, [_P, C.c_char_p, C.c_size_t]),
@@ -766,6 +772,7 @@ class MapContext:
                       ("total_counts", np.uint64)):
             out[k] = np.ctypeslib.as_array(getattr(r, k), shape=(M,)).copy() if M else np.zeros(0, dt)
         out["lib_format_counts"] = dict(zip(("ISF", "ISR", "SF", "SR"), [int(x) for x in r.lib_format_counts[:4]]))
+        out["rescue"] = {k: int(getattr(r, k)) for k in ("orphans_rescued", "rescue_searches", "rescue_no_room")}
         return out
 
     def online_state(self):
@@ -786,6 +793,24 @@ class MapContext:
             self.close()
         except Exception:
             pass
+
+
+def rescue_search_tap(patterns, windows, K, device=0):
+    """sb_rescue_search_tap: the orphan rescue's bit-vector infix search on the GPU.  patterns / windows: lists of uint8
+    code arrays (0..3, 4 = N), K: edit limits.  Returns (dist, end) int32 arrays, -1 where nothing is within K."""
+    n = len(patterns)
+    def cat(xs):
+        off = np.zeros(n + 1, dtype=np.uint64)
+        off[1:] = np.cumsum([len(x) for x in xs], dtype=np.uint64)
+        blob = np.ascontiguousarray(np.concatenate([np.asarray(x, dtype=np.uint8) for x in xs] + [np.zeros(1, np.uint8)]))
+        return blob, off
+    pb, po = cat(patterns)
+    wb, wo = cat(windows)
+    k = np.ascontiguousarray(K, dtype=np.int32)
+    dist = np.zeros(n, dtype=np.int32); end = np.zeros(n, dtype=np.int32)
+    _check(load().sb_rescue_search_tap(device, n, pb.ctypes.data, po.ctypes.data, wb.ctypes.data, wo.ctypes.data,
+                                       k.ctypes.data, dist.ctypes.data, end.ctypes.data), "sb_rescue_search_tap")
+    return dist, end
 
 
 # ------------------------------------------------------------------------------ SAM output

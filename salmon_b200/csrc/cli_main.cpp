@@ -75,6 +75,7 @@ int usage() {
           "  sb_salmon index -t transcripts.fa[.gz] -i index_dir [-k 31] [--gencode] [-d decoys.txt] [--keepDuplicates] [--no-clip]\n"
           "  sb_salmon quant -i index_dir -l IU|ISF|ISR -1 r1.fq[.gz] ... -2 r2.fq[.gz] ... | -l U|SF|SR -r reads.fq[.gz] ...  -o out_dir [--gpus N]\n"
           "                  [-p threads] [--dumpEq] [--dumpEqWeights] [--writeMappings[=FILE] | -z] [--writeQualities] [--writeUnmappedNames]\n"
+          "                  [--recoverOrphans]\n"
           "                  [--numBootstraps N | --numGibbsSamples N] [--thinningFactor 16] [--noGammaDraw] [--useEM] [--vbPrior 0.01]\n"
           "                  [--perNucleotidePrior] [--maxReadOcc 200] [--maxOccsPerHit 1000] [--minScoreFraction 0.65] [--consensusSlack 0.35]\n"
           "                  [--preMergeChainSubThresh 0.75] [--postMergeChainSubThresh 0.9] [--orphanChainSubThresh 0.95] [--allowDovetail]\n"
@@ -273,8 +274,9 @@ int cmd_quant(Args& a) {
     else if (o.rfind("--writeMappings=", 0) == 0) sam_path = o.substr(16);
     else if (o == "--writeQualities") qo.write_qualities = 1;
     else if (o == "--writeUnmappedNames") qo.write_unmapped_names = 1;
+    else if (o == "--recoverOrphans") mp.recover_orphans = 1;
     else if (o == "--seqBias" || o == "--gcBias" || o == "--posBias" || o == "-a" ||
-             o == "--alignments" || o == "--recoverOrphans" || o == "-g" || o == "--geneMap" || o == "--sketchMode") {
+             o == "--alignments" || o == "-g" || o == "--geneMap" || o == "--sketchMode") {
       fprintf(stderr, "sb_salmon quant: %s is outside the hot path this build replaces (DESIGN.md, out of scope)\n", o.c_str());
       return 1;
     } else { fprintf(stderr, "sb_salmon quant: unknown option %s\n", o.c_str()); return usage(); }
@@ -377,6 +379,7 @@ int cmd_quant(Args& a) {
   }
   mp.lib_type = lib_id;
   if (se_input && !pre_merge_given) mp.pre_merge_thresh = 1.0;    // single-end default (QuantOptionsUtils.cpp:215-218)
+  if (se_input) mp.recover_orphans = 0;   // a single-end read has no mate to rescue: accepted, no effect (as in salmon)
   // the CUDA context comes up (seconds) while the index is read from disk
   const double t_start = now_wall();
   std::thread ctx_thread([&] { sb_device_init(qo.device); });
@@ -400,6 +403,10 @@ int cmd_quant(Args& a) {
     fprintf(stderr, "mapping %.2f s (%.1f ms on the device, %.2f M fragments/s end to end, %d GPU(s)), optimiser %u iterations in %.2f s, total %.2f s; mapping set-up %.2f s\n",
             sum.map_seconds, sum.map_device_ms, sum.map_seconds > 0 ? (double)sum.n_observed / sum.map_seconds / 1e6 : 0.0, n_gpus, sum.em_iters,
             sum.em_seconds, sum.total_seconds, (double)sum.map_setup_ms * 1e-3);
+    if (mp.recover_orphans)
+      fprintf(stderr, "Number of orphans recovered using orphan rescue : %llu%s (%llu mate searches, %llu without room)\n",
+              (unsigned long long)sum.orphans_rescued, n_gpus > 1 ? " on rank 0" : "", (unsigned long long)sum.rescue_searches,
+              (unsigned long long)sum.rescue_no_room);
   }
   if (qo.shard_index == 0) fprintf(stderr, "done %.2f s after the process started\n", now_wall() - T_PROCESS_START);
   // the outputs are written and closed: leave without tearing down 10+ GB of host and device state piece by piece

@@ -21,6 +21,7 @@
 #include "common.cuh"
 #include "map_core.h"
 #include "map_kernels.cuh"
+#include "rescue.cuh"
 #include "sam_internal.h"
 
 using namespace sbmap;
@@ -549,11 +550,12 @@ __global__ void k_assign_work(uint32_t n, const uint32_t* __restrict__ n_l, cons
 }
 
 // SAM: a sink is attached -- also fill the side output (per-mate scores, decoy alignments); `side` holds the chunk's
-// base pointers.  The instance without it is the default path, unchanged.
-template <bool SAM>
+// base pointers.  RESCUE: orphan rescue ran on the chunk -- a read with rescued pairs takes them (rb) instead of the
+// join.  The instance without either is the default path, unchanged.
+template <bool SAM, bool RESCUE>
 __global__ void k_assign(IndexView ix, Params p, FldView fld, int useAux, int burnedIn, uint32_t n, uint32_t L,
                          BatchBufs b, OnlineView on, uint32_t chunk_first_read, const uint32_t* __restrict__ order,
-                         SamSide side) {
+                         SamSide side, RescueBufs rb) {
   const uint32_t T = gridDim.x * blockDim.x;
   const uint32_t tid0 = blockIdx.x * blockDim.x + threadIdx.x;
   const uint32_t cap = p.max_read_occ;
@@ -592,14 +594,19 @@ __global__ void k_assign(IndexView ix, Params p, FldView fld, int useAux, int bu
       const Cand* gr = b.cand_r + (size_t)r * MAXCAND;
       for (uint32_t a = 0; a < nl; ++a) { lcl[a] = gl[a]; sl[a] = b.score_l[(size_t)r * MAXCAND + a]; }
       for (uint32_t a = 0; a < nr; ++a) { rcl[a] = gr[a]; sr[a] = b.score_r[(size_t)r * MAXCAND + a]; }
+      // rescued pairs (at most one per appended candidate, so <= 32 here) are built in place in jh
+      const uint32_t npre = RESCUE ? rescued_joints(p, rb, r, lcl, rcl, L, jh) : 0;
       assign_read(ix, p, fld, useAux != 0, burnedIn != 0, lcl, nl, rcl, nr, sl, sr, L, sc, pi, pt, b1, b2, b3, jh, o, ctr,
-                  &on, chunk_first_read + r, lp, sdp);
+                  &on, chunk_first_read + r, lp, sdp, npre ? jh : nullptr, npre);
     } else {
       const size_t so = (size_t)tid0 * cap;
-      assign_read(ix, p, fld, useAux != 0, burnedIn != 0, b.cand_l + (size_t)r * MAXCAND, nl,
-                  b.cand_r + (size_t)r * MAXCAND, nr, b.score_l + (size_t)r * MAXCAND,
+      const Cand* gl = b.cand_l + (size_t)r * MAXCAND;
+      const Cand* gr = b.cand_r + (size_t)r * MAXCAND;
+      const uint32_t npre = RESCUE ? rescued_joints(p, rb, r, gl, gr, L, b.jh + so) : 0;   // <= anchors <= cap
+      assign_read(ix, p, fld, useAux != 0, burnedIn != 0, gl, nl, gr, nr, b.score_l + (size_t)r * MAXCAND,
                   b.score_r + (size_t)r * MAXCAND, L, b.sc + so, b.perm_idx + so, b.perm_tid + so, b.bs_tid + so,
-                  b.bs_score + so, b.bs_idx + so, b.jh + so, o, ctr, &on, chunk_first_read + r, b.lp + so, sdp);
+                  b.bs_score + so, b.bs_idx + so, b.jh + so, o, ctr, &on, chunk_first_read + r, b.lp + so, sdp,
+                  npre ? b.jh + so : nullptr, npre);
     }
   }
   add_counters(b.ctr, ctr);
@@ -1038,6 +1045,12 @@ struct sb_map_ctx {
   sb_sam* sam = nullptr;
   SamDev* samd = nullptr;
   uint64_t sam_window = 256ull << 20;
+  // orphan rescue (p.recover_orphans): task lists of one chunk; the pair lists k_assign reads exist twice (alt set)
+  RescueBufs rb{};
+  uint32_t* alt_rs_n_pairs = nullptr;
+  uint16_t* alt_rs_pairs = nullptr;
+  uint64_t rescued_total = 0, rescue_searches_total = 0, rescue_no_room_total = 0;
+  std::vector<cudaEvent_t> ev_rescue;   // pairs of events around the rescue kernels of each chunk
 };
 
 template <typename T>
@@ -1161,7 +1174,7 @@ extern "C" sb_map_ctx* sb_map_create(sb_index* ix, const sb_map_params* q, int d
   p.seed = q->seed; p.mini_batch = q->mini_batch ? q->mini_batch : 5000; p.reserved = 0;
   p.pre_merge_thresh = q->pre_merge_thresh; p.post_merge_thresh = q->post_merge_thresh; p.orphan_thresh = q->orphan_thresh;
   p.allow_dovetail = q->allow_dovetail; p.allow_orphans = q->allow_orphans;
-  p.lib_type = q->lib_type; p.reserved3 = 0;
+  p.lib_type = q->lib_type; p.recover_orphans = q->recover_orphans ? 1 : 0;
   if (p.lib_type < 0 || p.lib_type > 5) { sb::set_error("unsupported library type %d (IU, ISF, ISR, U, SF, SR)", p.lib_type); delete c; return nullptr; }
   if (!(p.pre_merge_thresh >= 0 && p.pre_merge_thresh <= 1) || !(p.post_merge_thresh >= 0 && p.post_merge_thresh <= 1) ||
       !(p.orphan_thresh >= 0 && p.orphan_thresh <= 1)) {
@@ -1263,6 +1276,13 @@ extern "C" sb_map_ctx* sb_map_create(sb_index* ix, const sb_map_params* q, int d
   c->fld.cmf_cached = c->d_fld + 2 * n; c->fld.cmf_quirk = c->d_fld + 3 * n;
   cudaMemset(b.ctr, 0, sizeof(Counters));
   cudaMemset(c->d_full_dp, 0, 8);
+  if (p.recover_orphans) {
+    RescueBufs& r = c->rb;
+    const size_t NT = CH * 2 * MAXCAND;
+    A(&r.n_tasks, 1); A(&r.tasks, NT); A(&r.first, CH); A(&r.n_anchor, CH); A(&r.diag, NT); A(&r.score, NT);
+    A(&r.pairs, NT); A(&r.n_pairs, CH); A(&r.ctr, 3); A(&c->alt_rs_pairs, NT); A(&c->alt_rs_n_pairs, CH);
+    if (rc != SB_OK) { sb_map_destroy(c); return nullptr; }
+  }
   return c;
 }
 
@@ -1282,6 +1302,13 @@ extern "C" void sb_map_destroy(sb_map_ctx* c) {
   for (void* p : ptrs) cudaFree(p);
   cudaFree(c->d_dummy_mate);
   sam_dev_destroy(c->samd);
+  {
+    const RescueBufs& r = c->rb;
+    void* rp[] = {r.n_tasks, r.tasks, r.first, r.n_anchor, r.diag, r.score, r.pairs, r.n_pairs, r.ctr, c->alt_rs_pairs,
+                  c->alt_rs_n_pairs};
+    for (void* q : rp) cudaFree(q);
+    for (cudaEvent_t e : c->ev_rescue) cudaEventDestroy(e);
+  }
   cudaFree(c->alt_n_l); cudaFree(c->alt_n_r); cudaFree(c->alt_cand_l); cudaFree(c->alt_cand_r); cudaFree(c->alt_score_l); cudaFree(c->alt_score_r);
   for (int s = 0; s < 2; ++s) { if (c->ev_dp[s]) cudaEventDestroy(c->ev_dp[s]); if (c->ev_asg[s]) cudaEventDestroy(c->ev_asg[s]); }
   if (c->assign_stream) cudaStreamDestroy(c->assign_stream);
@@ -1298,7 +1325,11 @@ extern "C" void sb_map_destroy(sb_map_ctx* c) {
 
 extern "C" int sb_map_set_option(sb_map_ctx* c, const char* key, int64_t value) {
   if (!c || !key) { sb::set_error("null argument"); return SB_ERR_INVALID; }
-  if (!strcmp(key, "variant")) { c->variant = (int)value; return SB_OK; }
+  if (!strcmp(key, "variant")) {
+    if (value == 0 && c->p.recover_orphans) { sb::set_error("recover_orphans needs the warp kernels (variant 1)"); return SB_ERR_INVALID; }
+    c->variant = (int)value;
+    return SB_OK;
+  }
   if (!strcmp(key, "fast_dp")) { c->fast_ok = value ? 1 : 0; return SB_OK; }
   if (!strcmp(key, "input_on_device")) { c->input_dev = value ? 1 : 0; return SB_OK; }
   if (!strcmp(key, "ascii_reads")) {
@@ -1449,6 +1480,7 @@ static int map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, u
   SB_CUDA(cudaEventRecord(c->ev0, st));
   SB_CUDA(cudaMemsetAsync(c->b.ctr, 0, sizeof(Counters), st));
   SB_CUDA(cudaMemsetAsync(c->d_full_dp, 0, 8, st));
+  if (c->rb.ctr) SB_CUDA(cudaMemsetAsync(c->rb.ctr, 0, 24, st));
   // chunks: the host->device copy of chunk i+1 (copy stream) overlaps the kernels of chunk i
   const uint32_t CH = c->chunk;
   const uint32_t nch = (n + CH - 1) / CH;
@@ -1512,6 +1544,27 @@ static int map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, u
       }
       c->launches += 5;
     }
+    // orphan rescue: after the DP scores, before k_assign (and before the input buffers are handed back)
+    const bool resc = p.recover_orphans && !single_end;
+    RescueBufs rb = c->rb;
+    if (resc) {
+      if (ovl && set) { rb.pairs = c->alt_rs_pairs; rb.n_pairs = c->alt_rs_n_pairs; }
+      while (c->ev_rescue.size() < 2 * (size_t)(ch + 1)) { cudaEvent_t e; cudaEventCreate(&e); c->ev_rescue.push_back(e); }
+      SB_CUDA(cudaEventRecord(c->ev_rescue[2 * ch], st));
+      SB_CUDA(cudaMemsetAsync(rb.n_tasks, 0, 4, st));
+      k_rescue_select<<<nblk(cn, 128), 128, 0, st>>>(p, cn, L, bc.n_l, bc.n_r, bc.cand_l, bc.cand_r, bc.score_l, bc.score_r, rb);
+      const unsigned sb = c->n_sm * 8;
+      switch ((L + 63) / 64) {
+        case 1: k_rescue_search<1><<<sb, 128, 0, st>>>(ix, p, c->pr, L, bc.cand_l, bc.cand_r, rb); break;
+        case 2: k_rescue_search<2><<<sb, 128, 0, st>>>(ix, p, c->pr, L, bc.cand_l, bc.cand_r, rb); break;
+        case 3: k_rescue_search<3><<<sb, 128, 0, st>>>(ix, p, c->pr, L, bc.cand_l, bc.cand_r, rb); break;
+        default: k_rescue_search<4><<<sb, 128, 0, st>>>(ix, p, c->pr, L, bc.cand_l, bc.cand_r, rb); break;
+      }
+      k_rescue_score<<<c->n_sm * 4, 256, 0, st>>>(ix, p, dl, dr, L, c->ascii, bc.cand_l, bc.cand_r, rb);
+      k_rescue_commit<<<nblk(cn, 128), 128, 0, st>>>(p, cn, L, bc.n_l, bc.n_r, bc.cand_l, bc.cand_r, bc.score_l, bc.score_r, rb);
+      SB_CUDA(cudaEventRecord(c->ev_rescue[2 * ch + 1], st));
+      c->launches += 4;
+    }
     cudaStream_t as = st;
     if (ovl) {   // the input staging buffers are free once the DP kernels are done; k_assign moves to its own stream
       SB_CUDA(cudaEventRecord(c->ev_free[s], st));
@@ -1527,9 +1580,11 @@ static int map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, u
     if (sam) {
       SamSide sd = sam_dev_side(c->samd);
       sd.n_out += c0; sd.decoy += c0; sd.score1 += (size_t)c0 * cap; sd.score2 += (size_t)c0 * cap;
-      k_assign<true><<<T / 128, 128, 0, as>>>(ix, p, c->fld, useAux, burnedIn, cn, L, bc, onv, c0, c->d_order, sd);
+      if (resc) k_assign<true, true><<<T / 128, 128, 0, as>>>(ix, p, c->fld, useAux, burnedIn, cn, L, bc, onv, c0, c->d_order, sd, rb);
+      else k_assign<true, false><<<T / 128, 128, 0, as>>>(ix, p, c->fld, useAux, burnedIn, cn, L, bc, onv, c0, c->d_order, sd, rb);
     } else {
-      k_assign<false><<<T / 128, 128, 0, as>>>(ix, p, c->fld, useAux, burnedIn, cn, L, bc, onv, c0, c->d_order, SamSide{});
+      if (resc) k_assign<false, true><<<T / 128, 128, 0, as>>>(ix, p, c->fld, useAux, burnedIn, cn, L, bc, onv, c0, c->d_order, SamSide{}, rb);
+      else k_assign<false, false><<<T / 128, 128, 0, as>>>(ix, p, c->fld, useAux, burnedIn, cn, L, bc, onv, c0, c->d_order, SamSide{}, rb);
     }
     c->launches += 3;
     if (ovl) SB_CUDA(cudaEventRecord(c->ev_asg[set], as));
@@ -1561,6 +1616,8 @@ static int map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, u
   unsigned long long full_dp = 0;
   SB_CUDA(cudaMemcpyAsync(&h, b.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaMemcpyAsync(&full_dp, c->d_full_dp, 8, cudaMemcpyDeviceToHost, st));
+  unsigned long long rctr[3] = {0, 0, 0};
+  if (c->rb.ctr) SB_CUDA(cudaMemcpyAsync(rctr, c->rb.ctr, 24, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaEventRecord(c->ev1, st));
   const double t_enq = wall_s();
   SB_CUDA(cudaEventSynchronize(c->ev1));
@@ -1574,6 +1631,7 @@ static int map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, u
   c->frags_seen += n;
   c->timestep += nsteps;
   c->full_dp_total += full_dp;
+  c->rescued_total += rctr[0]; c->rescue_searches_total += rctr[1]; c->rescue_no_room_total += rctr[2];
   if (!c->burned_in && c->frag_counter >= p.num_burnin) {   // SalmonQuantify.cpp:1013-1018
     k_online_correction<<<1, 32, 0, st>>>(c->nf, c->on, 1, c->d_scratch_nf, c->d_fld + c->nf, c->d_fld + 2 * (size_t)c->nf);
     if (c->M) k_online_eff_len<<<nblk(c->M, 256), 256, 0, st>>>(c->M, c->nf, c->index->d_tx_off, c->on.cf, c->on.log_eff);
@@ -1598,6 +1656,13 @@ static int map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, u
         if (cudaEventElapsedTime(&ms, c->ev_seed[2 * ch], c->ev_seed[2 * ch + 1]) == cudaSuccess) {
           stats->seed_kernel_ms += ms; stats->seed_kernel_launches++;
         }
+      }
+    stats->orphans_rescued = rctr[0]; stats->rescue_searches = rctr[1]; stats->rescue_no_room = rctr[2];
+    stats->rescue_kernel_ms = 0;
+    if (c->p.recover_orphans && !single_end)
+      for (uint32_t ch = 0; ch < nch; ++ch) {
+        float ms = 0;
+        if (cudaEventElapsedTime(&ms, c->ev_rescue[2 * ch], c->ev_rescue[2 * ch + 1]) == cudaSuccess) stats->rescue_kernel_ms += ms;
       }
   }
   return SB_OK;
@@ -1653,6 +1718,59 @@ extern "C" int sb_detect_lib_type(int paired, const uint64_t counts4[4]) {
   if (ratio < 0.3) return paired ? SB_LIB_ISR : SB_LIB_SR;
   if (ratio < 0.7) return paired ? SB_LIB_IU : SB_LIB_U;
   return paired ? SB_LIB_ISF : SB_LIB_SF;
+}
+
+// parity tap of the rescue search: the windows are laid out as the index lays out its reference (2-bit packed behind a
+// guard, byte codes for windows with N) and searched by the device function k_rescue_search runs
+extern "C" int sb_rescue_search_tap(int device, uint32_t n, const uint8_t* pats, const uint64_t* pat_off,
+                                    const uint8_t* wins, const uint64_t* win_off, const int32_t* K, int32_t* dist,
+                                    int32_t* end) {
+  if (n && (!pats || !pat_off || !wins || !win_off || !K || !dist || !end)) { sb::set_error("null argument"); return SB_ERR_INVALID; }
+  for (uint32_t i = 0; i < n; ++i)
+    if (pat_off[i + 1] < pat_off[i] || pat_off[i + 1] - pat_off[i] > 64 * RESCUE_MAX_WORDS || win_off[i + 1] < win_off[i]) {
+      sb::set_error("sb_rescue_search_tap: case %u: patterns of 0..%u bases", i, 64 * RESCUE_MAX_WORDS);
+      return SB_ERR_INVALID;
+    }
+  if (!n) return SB_OK;
+  SB_CUDA(cudaSetDevice(device));
+  const uint64_t np = pat_off[n], nw = win_off[n];
+  std::vector<uint64_t> packed((nw + 2 * (uint64_t)PACK_GUARD_BASES + 31) / 32 + 2, 0);
+  std::vector<uint8_t> has_n(n, 0);
+  for (uint32_t i = 0; i < n; ++i)
+    for (uint64_t g = win_off[i]; g < win_off[i + 1]; ++g) {
+      if (wins[g] > 3) { has_n[i] = 1; continue; }
+      const uint64_t q = g + PACK_GUARD_BASES;
+      packed[q >> 5] |= (uint64_t)wins[g] << (2 * (q & 31));
+    }
+  uint8_t *d_p = nullptr, *d_w = nullptr, *d_hn = nullptr;
+  uint64_t *d_po = nullptr, *d_wo = nullptr, *d_pk = nullptr;
+  int32_t *d_k = nullptr, *d_d = nullptr, *d_e = nullptr;
+  int rc = SB_OK;
+  auto A = [&](auto** ptr, size_t m) { if (rc == SB_OK) rc = dmalloc(ptr, m); };
+  A(&d_p, np); A(&d_w, nw); A(&d_hn, n); A(&d_po, n + 1); A(&d_wo, n + 1); A(&d_pk, packed.size()); A(&d_k, n);
+  A(&d_d, n); A(&d_e, n);
+  cudaError_t e = cudaSuccess;
+  if (rc == SB_OK) {
+    cudaMemcpy(d_p, pats, np, cudaMemcpyHostToDevice); cudaMemcpy(d_w, wins, nw, cudaMemcpyHostToDevice);
+    cudaMemcpy(d_hn, has_n.data(), n, cudaMemcpyHostToDevice); cudaMemcpy(d_po, pat_off, (n + 1) * 8, cudaMemcpyHostToDevice);
+    cudaMemcpy(d_wo, win_off, (n + 1) * 8, cudaMemcpyHostToDevice);
+    cudaMemcpy(d_pk, packed.data(), packed.size() * 8, cudaMemcpyHostToDevice);
+    cudaMemcpy(d_k, K, (size_t)n * 4, cudaMemcpyHostToDevice);
+    cudaMemset(d_d, 0xff, (size_t)n * 4); cudaMemset(d_e, 0xff, (size_t)n * 4);
+    // one launch per word count: each case runs in the instance k_rescue_search uses for its pattern length
+    k_rescue_tap<1><<<nblk(n, 128), 128>>>(n, d_p, d_po, d_pk, d_w, d_wo, d_hn, d_k, d_d, d_e);
+    k_rescue_tap<2><<<nblk(n, 128), 128>>>(n, d_p, d_po, d_pk, d_w, d_wo, d_hn, d_k, d_d, d_e);
+    k_rescue_tap<3><<<nblk(n, 128), 128>>>(n, d_p, d_po, d_pk, d_w, d_wo, d_hn, d_k, d_d, d_e);
+    k_rescue_tap<4><<<nblk(n, 128), 128>>>(n, d_p, d_po, d_pk, d_w, d_wo, d_hn, d_k, d_d, d_e);
+    e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) e = cudaMemcpy(dist, d_d, (size_t)n * 4, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(end, d_e, (size_t)n * 4, cudaMemcpyDeviceToHost);
+  }
+  void* ptrs[] = {d_p, d_w, d_hn, d_po, d_wo, d_pk, d_k, d_d, d_e};
+  for (void* q : ptrs) cudaFree(q);
+  if (rc != SB_OK) return rc;
+  if (e != cudaSuccess) { sb::set_error("sb_rescue_search_tap: %s", cudaGetErrorString(e)); return SB_ERR_CUDA; }
+  return SB_OK;
 }
 
 // debug / parity tap: per-read alignments of the LAST batch (arrays sized n*cap, label n*2*cap)
@@ -1797,6 +1915,8 @@ extern "C" int sb_map_finish(sb_map_ctx* c, sb_map_result* out) {
   out->n_mapped = c->totals.mapped;
   memset(out->lib_format_counts, 0, sizeof(out->lib_format_counts));
   for (int i = 0; i < 4; ++i) out->lib_format_counts[i] = c->totals.lib_mask_sum[i];
+  out->orphans_rescued = c->rescued_total; out->rescue_searches = c->rescue_searches_total;
+  out->rescue_no_room = c->rescue_no_room_total;
   out->lookups = c->totals.lookups; out->postings = c->totals.postings; out->seeds = c->totals.seeds;
   out->candidates = c->totals.candidates; out->kept = c->totals.kept; out->label_entries = c->totals.label_entries;
   out->n_txps = c->M;
@@ -1892,6 +2012,7 @@ extern "C" int sb_map_reset(sb_map_ctx* c) {
   c->stores.clear();
   c->arena.n_l = c->arena.n_w = c->arena.n_c = c->arena.n_o = 0;
   c->frag_counter = 0; c->frags_seen = 0; c->timestep = 0; c->burned_in = 0; c->full_dp_total = 0;
+  c->rescued_total = 0; c->rescue_searches_total = 0; c->rescue_no_room_total = 0;
   memset(&c->totals, 0, sizeof(c->totals));
   const std::vector<double>& t = c->init_tables;
   SB_CUDA(cudaMemcpy(c->d_fld, t.data(), (size_t)4 * c->nf * 8, cudaMemcpyHostToDevice));

@@ -37,7 +37,8 @@ struct Params {
   uint32_t mini_batch, reserved;
   double pre_merge_thresh, post_merge_thresh, orphan_thresh;   // join policy (see sb_map_params)
   int32_t allow_dovetail, allow_orphans;
-  int32_t lib_type, reserved3;      // expected library format (SB_LIB_*)
+  int32_t lib_type;                 // expected library format (SB_LIB_*)
+  int32_t recover_orphans;          // --recoverOrphans (DESIGN.md §11); 0 = off
 };
 
 struct TableEntry {
@@ -473,6 +474,180 @@ SB_HD int32_t dp_score_serial(const IndexView& ix, const Params& p, const uint8_
   return best;
 }
 
+// ---- orphan rescue (--recoverOrphans; the rule is DESIGN.md §11).  For a read whose joint hits are orphans only, every
+// orphan that scores and would form a library-compatible pair is an anchor: the other mate is searched for (infix edit
+// distance, Myers / Hyyro bit-vector form) in the window a fragment of at most max_frag_len allows, and the place found
+// becomes a new candidate of that mate, scored by the same banded DP.
+constexpr uint32_t RESCUE_MAX_WORDS = 4;   // reads up to 256 bases
+
+// one mate's DP score passes the single-mate threshold (the hit-score rule of assign_read for one mate)
+SB_HD bool rescue_mate_passes(const Params& p, int32_t score, uint32_t L) {
+  return score > NEG_SCORE && (double)score >= p.min_score_fraction * (double)(p.ma * (int32_t)L);
+}
+// edit limit K: every edit costs at least min(ma - mp, ge) against a perfect score, so a place with more than K edits
+// cannot pass rescue_mate_passes
+SB_HD int32_t rescue_edit_limit(const Params& p, uint32_t L) {
+  const int32_t per = (p.ma - p.mp) < p.ge ? (p.ma - p.mp) : p.ge;
+  if (per <= 0) return (int32_t)L;
+  const double k = (1.0 - p.min_score_fraction) * (double)p.ma * (double)L / (double)per;
+  if (!(k >= 0)) return 0;
+  return k >= (double)L ? (int32_t)L : (int32_t)k;
+}
+// anchor side 0 = left mate, 1 = right mate: the pair the anchor would form is compatible with the library type
+SB_HD bool rescue_anchor_ok(const Params& p, const Cand& a, uint32_t side, int32_t score, uint32_t L) {
+  const bool afw = (a.ori_cov >> 31) == 0;
+  const bool lfw = side == 0 ? afw : !afw, rfw = side == 0 ? !afw : afw;
+  return rescue_mate_passes(p, score, L) && lib_compatible(p.lib_type, 0, lfw, rfw);
+}
+// search window [lo, hi) on the anchor's transcript (length tlen); false if empty after clipping
+SB_HD bool rescue_window(const Params& p, const Cand& a, uint32_t L, int64_t tlen, int64_t& lo, int64_t& hi) {
+  const int64_t d = a.diag_c, F = (int64_t)p.max_frag_len;
+  if ((a.ori_cov >> 31) == 0) { lo = d; hi = d + F; }
+  else { lo = d + (int64_t)L - F; hi = d + (int64_t)L; }
+  if (lo < 0) lo = 0;
+  if (hi > tlen) hi = tlen;
+  return hi > lo;
+}
+// base i of the pattern searched for: the other mate as given (anchor reverse) or its reverse complement (anchor forward)
+SB_HD uint8_t rescue_pattern_base(const uint8_t* mate, uint32_t L, bool rc, uint32_t i) {
+  if (!rc) return mate[i];
+  const uint8_t c = mate[L - 1 - i];
+  return c > 3 ? (uint8_t)4 : (uint8_t)(3 - c);
+}
+
+// Infix (semi-global) edit distance of pattern P (m <= 64*NW bases, code 4 matches nothing) against text(0..n-1)
+// (a functor returning the code of text base j, called with j = 0, 1, ... in order): the smallest distance over all
+// end positions and the leftmost end at that distance; dist = end = -1 when the smallest distance exceeds K.
+// Column-wise bit-vector recurrence (Myers 1999, Hyyro's block form); the free start is a zero top row.
+template <uint32_t NW, class PatF, class TextF>
+SB_HD void myers_infix(PatF&& pat, uint32_t m, uint32_t n, TextF&& text, int32_t K, int32_t& dist, int32_t& end) {
+  uint64_t peq[4][NW], Pv[NW], Mv[NW];
+#pragma unroll
+  for (uint32_t w = 0; w < NW; ++w) { peq[0][w] = peq[1][w] = peq[2][w] = peq[3][w] = 0; Pv[w] = ~0ull; Mv[w] = 0; }
+  for (uint32_t i = 0; i < m; ++i) {
+    const uint8_t c = pat(i);
+    const uint64_t bit = 1ull << (i & 63);
+#pragma unroll
+    for (uint32_t w = 0; w < NW; ++w)
+      if ((i >> 6) == w) {
+        if (c == 0) peq[0][w] |= bit;
+        else if (c == 1) peq[1][w] |= bit;
+        else if (c == 2) peq[2][w] |= bit;
+        else if (c == 3) peq[3][w] |= bit;
+      }
+  }
+  const uint32_t last = (m - 1) >> 6, hb = (m - 1) & 63;
+  int32_t score = (int32_t)m, best = K + 1, bend = -1;
+  for (uint32_t j = 0; j < n; ++j) {
+    const uint8_t c = text(j);
+    int32_t hin = 0;   // horizontal delta entering the block from above (row -1 is all zeros: free start)
+#pragma unroll
+    for (uint32_t w = 0; w < NW; ++w) {
+      if (w > last) break;
+      uint64_t eq = c == 0 ? peq[0][w] : c == 1 ? peq[1][w] : c == 2 ? peq[2][w] : c == 3 ? peq[3][w] : 0ull;
+      const uint64_t pv = Pv[w], mv = Mv[w];
+      const uint64_t hneg = hin < 0 ? 1ull : 0ull, hpos = hin > 0 ? 1ull : 0ull;
+      const uint64_t xv = eq | mv;
+      eq |= hneg;
+      const uint64_t xh = (((eq & pv) + pv) ^ pv) | eq;
+      uint64_t ph = mv | ~(xh | pv);
+      uint64_t mh = pv & xh;
+      if (w == last) score += (int32_t)((ph >> hb) & 1ull) - (int32_t)((mh >> hb) & 1ull);
+      hin = (int32_t)(ph >> 63) - (int32_t)(mh >> 63);
+      ph = (ph << 1) | hpos;
+      mh = (mh << 1) | hneg;
+      Pv[w] = mh | ~(xv | ph);
+      Mv[w] = ph & xv;
+    }
+    if (score < best) { best = score; bend = (int32_t)j; }
+  }
+  dist = bend >= 0 ? best : -1;
+  end = bend;
+}
+template <class PatF, class TextF>
+SB_HD void myers_infix_any(PatF&& pat, uint32_t m, uint32_t n, TextF&& text, int32_t K, int32_t& dist, int32_t& end) {
+  if (m <= 64) myers_infix<1>(pat, m, n, text, K, dist, end);
+  else if (m <= 128) myers_infix<2>(pat, m, n, text, K, dist, end);
+  else if (m <= 192) myers_infix<3>(pat, m, n, text, K, dist, end);
+  else myers_infix<4>(pat, m, n, text, K, dist, end);
+}
+
+// The search of one anchor with the byte codes of the index (host form; the kernel streams the 2-bit packed reference).
+// Returns the rescued candidate's diagonal through diag; false when the window is empty or nothing is within K.
+SB_HD bool rescue_search_serial(const IndexView& ix, const Params& p, const Cand& a, const uint8_t* mate, uint32_t L,
+                                int32_t& diag) {
+  const int64_t tlen = (int64_t)(ix.tx_off[a.tid + 1] - ix.tx_off[a.tid]);
+  int64_t lo, hi;
+  if (!rescue_window(p, a, L, tlen, lo, hi)) return false;
+  const uint8_t* ref = ix.codes + ix.tx_off[a.tid] + lo;
+  const bool rc = (a.ori_cov >> 31) == 0;
+  int32_t dist, end;
+  myers_infix_any([&](uint32_t i) { return rescue_pattern_base(mate, L, rc, i); }, L, (uint32_t)(hi - lo),
+                  [&](uint32_t j) { return ref[j]; }, rescue_edit_limit(p, L), dist, end);
+  if (dist < 0) return false;
+  diag = (int32_t)(lo + end) - (int32_t)L + 1;
+  return true;
+}
+
+// Anchors of one read, in joint order (side: 0 left / 1 right, ci: candidate index).  None unless the read's joint hits
+// are orphans only and 1 <= nj <= max_read_occ.  side / ci: room for 2 * MAXCAND entries.
+SB_HD uint32_t rescue_anchors(const Params& p, const Cand* lc, uint32_t nl, const Cand* rc, uint32_t nr, const int32_t* sl,
+                              const int32_t* sr, uint32_t L, uint8_t* side, uint8_t* ci) {
+  bool paired = false;
+  const uint32_t nj = for_each_joint(p, lc, nl, rc, nr, L, [&](const Joint& j, uint32_t) { paired |= j.status == 0; });
+  if (paired || nj == 0 || nj > p.max_read_occ) return 0;
+  uint32_t na = 0;
+  for_each_joint(p, lc, nl, rc, nr, L, [&](const Joint& j, uint32_t) {
+    const uint32_t s = j.status == 1 ? 0u : 1u;
+    const int32_t c = s == 0 ? j.li : j.ri;
+    if (rescue_anchor_ok(p, s == 0 ? lc[c] : rc[c], s, s == 0 ? sl[c] : sr[c], L)) { side[na] = (uint8_t)s; ci[na] = (uint8_t)c; ++na; }
+  });
+  return na;
+}
+
+// The rescued candidate of an anchor: same transcript, opposite orientation.  Coverage 0 (the join never sees it).
+SB_HD Cand rescue_cand(const Cand& a, int32_t diag) {
+  Cand c;
+  c.tid = a.tid; c.diag_c = diag; c.ori_cov = (a.ori_cov >> 31) ? 0u : 0x80000000u;
+  return c;
+}
+
+// Commit of one read, anchors in joint order.  side / ci: anchor's mate (0 left) and candidate index; diag / score: the
+// place found and the rescued mate's DP score there (INVALID_SCORE: nothing within K).  Rescued candidates are appended to lc / rc (their scores
+// to sl / sr) while a list has room; the rescued pairs (status 0) go to out in anchor order, an identical pair (same
+// transcript, same (orientation, diagonal) for both mates) only once.  Returns the number of pairs; no_room counts the
+// anchors that found a valid mate but no room for it.
+SB_HD uint32_t rescue_commit(const Params& p, uint32_t L, Cand* lc, uint32_t& nl, Cand* rc, uint32_t& nr, int32_t* sl,
+                             int32_t* sr, uint32_t n_anchor, const uint8_t* side, const uint8_t* ci, const int32_t* diag, const int32_t* score, Joint* out, uint32_t& no_room) {
+  uint32_t np = 0;
+  for (uint32_t a = 0; a < n_anchor; ++a) {
+    if (!rescue_mate_passes(p, score[a], L)) continue;
+    const Cand anc = side[a] == 0 ? lc[ci[a]] : rc[ci[a]];
+    const Cand res = rescue_cand(anc, diag[a]);
+    const Cand& l = side[a] == 0 ? anc : res;
+    const Cand& r = side[a] == 0 ? res : anc;
+    int32_t fl;
+    if (!pair_geometry(p, l, r, L, fl)) continue;
+    bool dup = false;
+    for (uint32_t q = 0; q < np && !dup; ++q) {
+      const Cand& ql = lc[out[q].li];
+      const Cand& qr = rc[out[q].ri];
+      dup = ql.tid == l.tid && ql.diag_c == l.diag_c && (ql.ori_cov >> 31) == (l.ori_cov >> 31) &&
+            qr.diag_c == r.diag_c && (qr.ori_cov >> 31) == (r.ori_cov >> 31);
+    }
+    if (dup) continue;
+    uint32_t& n = side[a] == 0 ? nr : nl;
+    if (n >= (uint32_t)MAXCAND) { ++no_room; continue; }
+    Joint j;
+    j.tid = anc.tid; j.frag_len = fl; j.status = 0;
+    if (side[a] == 0) { rc[n] = res; sr[n] = score[a]; j.li = (int32_t)ci[a]; j.ri = (int32_t)n; }
+    else { lc[n] = res; sl[n] = score[a]; j.li = (int32_t)n; j.ri = (int32_t)ci[a]; }
+    ++n;
+    out[np++] = j;
+  }
+  return np;
+}
+
 // ---- salmon-owned arithmetic on the log scale (deterministic exp/log, sb_detmath.h)
 SB_HD double log0() { return sbm_u2d(0x7ff0000000000000ull); }   // LOG_0 = HUGE_VAL (SalmonMath.hpp:40)
 SB_HD double dabs(double x) { return x < 0 ? -x : x; }
@@ -578,16 +753,22 @@ SB_HD void assign_read(const IndexView& ix, const Params& p, const FldView& fld,
                        const int32_t* score_r, uint32_t L, int32_t* sc, int32_t* perm_idx, int32_t* perm_tid,
                        int32_t* bs_tid, int32_t* bs_score, int32_t* bs_idx, Joint* jh, const ReadOut& o,
                        Counters& ctr, const OnlineView* on = nullptr, uint32_t read_in_batch = 0,
-                       double* lpbuf = nullptr /* >= cap doubles */, const SamSide* side = nullptr) {
+                       double* lpbuf = nullptr /* >= cap doubles */, const SamSide* side = nullptr,
+                       const Joint* pre_joints = nullptr /* rescued pairs (rescue_commit) replace the join */,
+                       uint32_t n_pre = 0) {
   const double LOG_EPSILON = -24.006680182952184;   // log(0.375e-10), SalmonMath.hpp:44-45 (libm and sbm_det_log agree)
   const uint32_t cap = p.max_read_occ;
   *o.n_aln = 0;
   if (side) { *side->n_out = 0; *side->decoy = 0; }
   uint32_t nj = 0;
-  const uint32_t total = for_each_joint(p, lc, nl, rcd, nr, L, [&](const Joint& j, uint32_t k) {
-    if (k < cap) jh[k] = j;
-  });
-  nj = total;
+  if (pre_joints) {
+    for (uint32_t k = 0; k < n_pre && k < cap; ++k) jh[k] = pre_joints[k];
+    nj = n_pre;
+  } else {
+    nj = for_each_joint(p, lc, nl, rcd, nr, L, [&](const Joint& j, uint32_t k) {
+      if (k < cap) jh[k] = j;
+    });
+  }
   if (nj == 0 || nj > cap) return;
   // ---- SalmonMappingUtils.hpp:225-281
   int32_t bestScore = INVALID_SCORE, bestDecoyScore = INVALID_SCORE;

@@ -364,6 +364,7 @@ struct MetaIn {
   std::string files, start_time, end_time;
   int n_ranks;
   uint64_t lib_counts[4];     // fragments that showed ISF / ISR / SF / SR among their kept mappings
+  uint64_t orphans_rescued;   // over all ranks
 };
 std::string time_string() {
   time_t t = time(nullptr);
@@ -435,13 +436,15 @@ int write_run_metadata(const std::string& outs, const MetaIn& m) {
              "    \"length_classes\": [],\n    \"index_seq_hash\": \"\",\n    \"index_name_hash\": \"\",\n    \"num_bootstraps\": %u,\n"
              "    \"num_processed\": %llu,\n    \"num_mapped\": %llu,\n    \"num_decoy_fragments\": 0,\n    \"num_dovetail_fragments\": 0,\n"
              "    \"num_fragments_filtered_vm\": 0,\n    \"num_alignments_below_threshold_for_mapped_fragments_vm\": 0,\n"
-             "    \"percent_mapped\": %.6f,\n    \"call\": \"quant\",\n    \"start_time\": \"%s\",\n    \"end_time\": \"%s\",\n    \"sb_num_gpus\": %d\n}\n",
+             "    \"percent_mapped\": %.6f,\n    \"call\": \"quant\",\n    \"start_time\": \"%s\",\n    \"end_time\": \"%s\",\n    \"sb_num_gpus\": %d,\n"
+             "    \"sb_num_orphans_rescued\": %llu\n}\n",
              sb_version(), m.o->num_bootstraps ? "bootstrap" : (m.o->num_gibbs ? "gibbs" : "none"), m.ep->use_vbem ? "vb" : "em",
              (m.mp->lib_type >= 0 && m.mp->lib_type <= 5) ? (const char* const[]){"IU", "ISF", "ISR", "U", "SF", "SR"}[m.mp->lib_type] : "IU",
              pmf.size(), mean, sd, m.n_valid, m.n_decoy, (unsigned long long)m.n_classes,
              (m.o->dump_eq || m.o->dump_eq_weights) ? "true" : "false",
              m.mp->range_bins ? "\n        \"range_factorized\"\n    " : "", n_samp, (unsigned long long)m.n_observed,
-             (unsigned long long)m.n_mapped, pct, m.start_time.c_str(), m.end_time.c_str(), m.n_ranks);
+             (unsigned long long)m.n_mapped, pct, m.start_time.c_str(), m.end_time.c_str(), m.n_ranks,
+             (unsigned long long)m.orphans_rescued);
     ok = write_text(outs + "/aux_info/meta_info.json", buf) && ok;
   }
   {   // lib_format_counts.json (ReadExperiment.inl:219-350): every kept mapping is compatible with the expected format
@@ -730,8 +733,9 @@ extern "C" int sb_quant_files(sb_index* ix, const char* const* mates1, const cha
     names = np.data();
   }
   // (a collective: every rank takes part, whether it writes the outputs or not)
-  uint64_t libc[4] = {res.lib_format_counts[0], res.lib_format_counts[1], res.lib_format_counts[2], res.lib_format_counts[3]};
-  if (multi) SB_TRY(sb_comm_allreduce(S.comm, libc, 4, 1, 0));
+  uint64_t libc[5] = {res.lib_format_counts[0], res.lib_format_counts[1], res.lib_format_counts[2], res.lib_format_counts[3],
+                      res.orphans_rescued};
+  if (multi) SB_TRY(sb_comm_allreduce(S.comm, libc, 5, 1, 0));
   if (!outs.empty() && o.shard_index == 0) {
     if (!make_dirs(outs + "/aux_info")) { sb::set_error("cannot create %s/aux_info", outs.c_str()); return SB_ERR_INVALID; }
     std::vector<uint32_t> lens;
@@ -754,7 +758,7 @@ extern "C" int sb_quant_files(sb_index* ix, const char* const* mates1, const cha
       files += std::string(f ? ", " : "") + (mates2 ? std::string("( ") + mates1[f] + ", " + mates2[f] + " )" : std::string(mates1[f]));
     files += " ]";
     MetaIn mi{&o, &ep, &mp, Mq, M - Mq, n_observed, n_mapped_u, res.n_classes, &hist, glob.unique_counts, glob.total_counts,
-              files, start_time, time_string(), (int)o.shard_count, {libc[0], libc[1], libc[2], libc[3]}};
+              files, start_time, time_string(), (int)o.shard_count, {libc[0], libc[1], libc[2], libc[3]}, libc[4]};
     SB_TRY(write_run_metadata(outs, mi));
   }
   if (o.num_bootstraps || o.num_gibbs) {
@@ -771,6 +775,7 @@ extern "C" int sb_quant_files(sb_index* ix, const char* const* mates1, const cha
     sum->map_seconds = t_map - t0; sum->em_seconds = t_em - t_map; sum->total_seconds = now_s() - t0;
     sum->map_device_ms = device_ms;
     sum->map_setup_ms = (float)((t_setup - t0) * 1e3);
+    sum->orphans_rescued = res.orphans_rescued; sum->rescue_searches = res.rescue_searches; sum->rescue_no_room = res.rescue_no_room;
   }
   return SB_OK;
 }

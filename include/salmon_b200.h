@@ -593,24 +593,26 @@ int sb_reads_bucketed_meta(sb_reads* rd, uint32_t min_len, uint32_t batch, uint3
 
 /* Debug: per-warp phase timestamps (ns) of one iteration of the last persistent run:
  * out[n_warps*16] = {P1 start, P1 end, barrier1 end, P2 start, P2 end, reduce end, barrier2 end, P2 home stream end,
- * P1 home stream end, then per phase (P1, P2) what the warp took from the work queue: long rows << 32 | their entries,
- * tail tiles << 32 | their columns, longest row taken; -}.
+ * P1 home stream end, then per phase (slots 9-10 P1, 11-12 P2) what the warp took from the long-row work queue:
+ * long rows << 32 | their entries, longest row taken; -}.
  * Returns the number of warps (call with out=NULL to size the buffer). */
 int sb_em_debug_timeline(sb_em_ctx* ctx, uint64_t* out, uint32_t iteration);
 
-/* Tuning knobs (not part of the reference contract): kernel variant.
- * key: "variant" (0 = multi-kernel per iteration, 1 = persistent cooperative),
- *      "blocks_per_sm", "flush_l2_mb", "tail_pct" (0-100: share of each warp's slice range, by modelled work, that
- *      goes to the phase's work queue as tail tiles; 0 = static ranges), "tail_tile_cols" (least columns of a tile). */
+/* Tuning knobs (not part of the reference contract).  Unknown keys return SB_ERR_INVALID.
+ * key: "variant" (0 = multi-kernel per iteration, 1 = persistent cooperative), "blocks_per_sm" (0 = as many as fit),
+ *      "config" (kernel configuration 0-3: ring chunk x depth x resident blocks), "lmax" (longest row on the SELL path),
+ *      "lwarp" (longest row reduced by one warp), "sell_group_cm" / "sell_group_tm" (rows per length-bucketing group, a
+ *      power of two >= 32), "rebalance" (rounds of measured re-cutting of the warp ranges), "rebalance_iters",
+ *      "overhead_p1" / "overhead_p2" (per-slice epilogue cost in columns, for the range cut), "push_pass" (fused
+ *      multi-GPU path: -1 by rank count, 0 push from the row epilogues, 1 coalesced pass), "sample_offset". */
 int sb_em_set_option(sb_em_ctx* ctx, const char* key, int64_t value);
 
 /* Figures of the layout sb_em_prepare built (after prepare).  key: "stream_bytes" (bytes one iteration streams:
  * both SELL matrices at 10 bytes per entry, padding included, + the long rows' CSR at 12), or per matrix with the
  * suffix "_cm" (class-major) / "_tm" (transcript-major): "stream_bytes", "sell_cols" (SELL columns of 32 entries),
  * "long_rows", "long_entries", "fallback_rows" (rows on the long-row path only because their slice's indices span
- * more than 16 bits), "tail_tiles", "tail_cols" (tail tiles on the work queue and their SELL columns), "home_cols"
- * (SELL columns the warps stream through their rings; home_cols + tail_cols = sell_cols); "warps" (warps of the iteration grid, which the slice ranges were cut for), "ring_cols"
- * (columns one warp's stream ring holds). */
+ * more than 16 bits); "warps" (warps of the iteration grid, which the slice ranges were cut for), "ring_cols" (columns
+ * one warp's stream ring holds). */
 int sb_em_get_info(sb_em_ctx* ctx, const char* key, int64_t* value);
 
 /* ---- multi-GPU: classes stay sharded per rank, alpha is all-reduced once per

@@ -70,12 +70,7 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
       : "memory");
 }
 
-// L2 eviction-priority policies for the bulk copies (createpolicy + .L2::cache_hint)
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
+// L2 eviction-priority policy for the bulk copies (createpolicy + .L2::cache_hint)
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));

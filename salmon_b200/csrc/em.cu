@@ -9,11 +9,12 @@
 //   P1 (class-major):  denom_c = sum_i theta[t_i] * w_ci ;  scale_c = count_c / denom_c
 //   P2 (txp-major):    alpha'_t = base_t + theta_t * sum_c w_ct * scale_c
 //                      + convergence test + theta'_t (VBEM: exp(digamma(alpha'+prior) - logNorm))
-// Both passes stream fixed-size windows ("tiles") of the entry arrays into shared
+// Both passes stream each warp's range of the SELL-32 entry arrays into shared
 // memory with 1-D bulk (TMA) copies on an mbarrier ring and gather theta / scale
 // from L2.  A persistent cooperative kernel runs the whole iteration loop with two
-// grid barriers per iteration; the multi-kernel variant launches P1 / P2 separately
-// (used for the multi-GPU path where an all-reduce sits between P2 and the update).
+// grid barriers per iteration.  The per-phase kernels launch P1 and P2 (or P2's
+// partial alpha') separately: variant 0 on one GPU, and the NCCL multi-GPU path,
+// where an all-reduce sits between P2's partials and the update.
 #include <cooperative_groups.h>
 #include <cub/cub.cuh>
 #include <float.h>
@@ -360,13 +361,12 @@ __global__ void k_sell_fill(uint32_t n_rows, uint32_t n_slices, const uint32_t* 
 }
 // contiguous, work-balanced slice ranges per warp: work(slice) = width + overhead
 __global__ void k_warp_ranges(uint32_t n_slices, const uint32_t* __restrict__ slice_ptr,
-                              uint32_t overhead, uint32_t n_warps, const uint64_t* __restrict__ targets,
-                              uint32_t* __restrict__ warp_begin) {
+                              uint32_t overhead, uint32_t n_warps, uint32_t* __restrict__ warp_begin) {
   const uint32_t wid = blockIdx.x * blockDim.x + threadIdx.x;
   if (wid > n_warps) return;
   if (wid == n_warps || n_slices == 0) { warp_begin[wid] = n_slices; return; }
   const uint64_t total = (uint64_t)slice_ptr[n_slices] + (uint64_t)overhead * n_slices;
-  const uint64_t target = targets ? targets[wid] : total * wid / n_warps;
+  const uint64_t target = total * wid / n_warps;
   uint32_t lo = 0, hi = n_slices;  // first slice whose cumulative work (before it) >= target
   while (lo < hi) {
     uint32_t mid = (lo + hi) >> 1;
@@ -544,7 +544,6 @@ extern "C" sb_em_ctx* sb_em_create(int device) {
   // development overrides of the tuning defaults (sweeps over the test-suite)
   if (const char* e = getenv("SB_EM_CONFIG")) { const int v = atoi(e); if (v >= 0 && v < N_KERNEL_SETS) c->config = v; }
   if (const char* e = getenv("SB_EM_LWARP")) { const int v = atoi(e); if (v >= 1) c->lwarp = v; }
-  if (const char* e = getenv("SB_EM_BALANCE")) c->balance_long = atoi(e);
   if (const char* e = getenv("SB_EM_GROUP_CM")) { const int v = atoi(e); if (v >= 32 && !(v & (v - 1))) c->sell_group_cm = v; }
   if (const char* e = getenv("SB_EM_GROUP_TM")) { const int v = atoi(e); if (v >= 32 && !(v & (v - 1))) c->sell_group_tm = v; }
   return c;
@@ -552,9 +551,7 @@ extern "C" sb_em_ctx* sb_em_create(int device) {
 
 static void free_sell(SellDev& m) {
   void** ptrs[] = {(void**)&m.slice_ptr, (void**)&m.width, (void**)&m.base, (void**)&m.len, (void**)&m.idx,
-                   (void**)&m.w, (void**)&m.warp_begin, (void**)&m.home_end, (void**)&m.long_rows, (void**)&m.tiles,
-                   (void**)&m.targets,
-                   };
+                   (void**)&m.w, (void**)&m.warp_begin, (void**)&m.long_rows};
   for (void** p : ptrs) {
     if (*p) cudaFree(*p);
     *p = nullptr;
@@ -621,20 +618,11 @@ extern "C" int sb_em_set_option(sb_em_ctx* c, const char* key, int64_t value) {
   } else if (!strcmp(key, "lwarp")) {
     if (value < 1 || value > 1000000) { set_error("lwarp out of range"); return SB_ERR_INVALID; }
     c->lwarp = (int)value; c->prepared = false;
-  } else if (!strcmp(key, "balance_long")) { c->balance_long = (int)value; c->prepared = false;
-  } else if (!strcmp(key, "l2_keep_cm")) { c->keep_cm = (int)value; }
-  else if (!strcmp(key, "l2_keep_tm")) { c->keep_tm = (int)value; }
+  }
   else if (!strcmp(key, "push_pass")) { c->push_pass = (int)value; }
   else if (!strcmp(key, "sample_offset")) { c->sample_offset = (uint32_t)value; }
   else if (!strcmp(key, "rebalance")) { c->rebalance = (int)value; c->prepared = false; }
   else if (!strcmp(key, "rebalance_iters")) { c->rebalance_iters = (int)value; c->prepared = false; }
-  else if (!strcmp(key, "tail_pct")) {
-    if (value < 0 || value > 100) { set_error("tail_pct out of range"); return SB_ERR_INVALID; }
-    c->tail_pct = (int)value; c->prepared = false;
-  } else if (!strcmp(key, "tail_tile_cols")) {
-    if (value < 1 || value > 65536) { set_error("tail_tile_cols out of range"); return SB_ERR_INVALID; }
-    c->tail_tile_cols = (int)value; c->prepared = false;
-  }
   else if (!strcmp(key, "overhead_p1")) { c->ovh_p1 = (int)value; c->prepared = false; }
   else if (!strcmp(key, "overhead_p2")) { c->ovh_p2 = (int)value; c->prepared = false; }
   else { set_error("unknown option '%s'", key); return SB_ERR_INVALID; }
@@ -665,9 +653,6 @@ extern "C" int sb_em_get_info(sb_em_ctx* c, const char* key, int64_t* value) {
   else if (m && k == "long_rows") *value = m->n_long;
   else if (m && k == "long_entries") *value = (int64_t)m->long_entries;
   else if (m && k == "fallback_rows") *value = m->n_fallback;
-  else if (m && k == "tail_tiles") *value = m->n_tiles;
-  else if (m && k == "tail_cols") *value = (int64_t)m->tail_cols;
-  else if (m && k == "home_cols") *value = (int64_t)m->home_cols;
   else { set_error("unknown info key '%s'", key); return SB_ERR_INVALID; }
   return SB_OK;
 }
@@ -750,50 +735,6 @@ static double slice_cost(const std::vector<uint32_t>& sp, uint32_t s, uint32_t o
   return (double)(sp[s + 1] - sp[s]) + (sp[s + 1] > sp[s] ? (double)overhead : 0.0);
 }
 
-// Split every warp's slice range [s0, s1) at h: the home part [s0, h) carries (100 - tail_pct) % of the range's
-// modelled work and streams through the warp's ring; [h, s1) is cut at slice boundaries into tail tiles of at least
-// tail_tile_cols columns (a shorter rest joins the warp's previous tile), which the phase's work queue hands to
-// whichever warp is free after the long rows.  Every slice lies in exactly one home part or one tile.
-static int split_tails(sb_em_ctx* c, SellDev& m, uint32_t overhead, uint32_t n_warps) {
-  std::vector<uint32_t> sp((size_t)m.n_slices + 1), wb((size_t)n_warps + 1), home(std::max<uint32_t>(n_warps, 1));
-  SB_CUDA(cudaMemcpy(sp.data(), m.slice_ptr, sp.size() * 4, cudaMemcpyDeviceToHost));
-  SB_CUDA(cudaMemcpy(wb.data(), m.warp_begin, wb.size() * 4, cudaMemcpyDeviceToHost));
-  std::vector<uint4> tiles;
-  m.home_cols = m.tail_cols = 0;
-  for (uint32_t w = 0; w < n_warps; ++w) {
-    const uint32_t s0 = wb[w], s1 = wb[w + 1];
-    uint32_t h = s1;
-    if (c->tail_pct > 0) {
-      double work = 0.0;
-      for (uint32_t s = s0; s < s1; ++s) work += slice_cost(sp, s, overhead);
-      const double target = work * (100 - c->tail_pct) / 100.0;
-      double cum = 0.0;
-      for (h = s0; h < s1 && cum + 0.5 * slice_cost(sp, h, overhead) < target; ++h) cum += slice_cost(sp, h, overhead);
-    }
-    home[w] = h;
-    m.home_cols += sp[h] - sp[s0];
-    m.tail_cols += sp[s1] - sp[h];
-    const size_t first = tiles.size();
-    for (uint32_t t0 = h; t0 < s1;) {
-      uint32_t t1 = t0 + 1;
-      while (t1 < s1 && sp[t1] - sp[t0] < (uint32_t)c->tail_tile_cols) ++t1;
-      if (sp[t1] - sp[t0] < (uint32_t)c->tail_tile_cols && tiles.size() > first) {
-        tiles.back().y = t1;                   // a short rest joins the previous tile
-        tiles.back().w = sp[t1];
-      } else {
-        tiles.push_back(make_uint4(t0, t1, sp[t0], sp[t1]));
-      }
-      t0 = t1;
-    }
-  }
-  m.n_tiles = (uint32_t)tiles.size();
-  SB_TRY(dev_alloc(&m.home_end, home.size()));
-  SB_TRY(dev_alloc(&m.tiles, tiles.size()));
-  SB_CUDA(cudaMemcpy(m.home_end, home.data(), home.size() * 4, cudaMemcpyHostToDevice));
-  if (!tiles.empty()) SB_CUDA(cudaMemcpy(m.tiles, tiles.data(), tiles.size() * sizeof(uint4), cudaMemcpyHostToDevice));
-  return SB_OK;
-}
-
 // CSR (rows optionally permuted by rowperm) -> SELL-32 + long-row list + warp ranges
 static int build_sell(sb_em_ctx* c, SellDev& m, uint32_t n_rows, const uint32_t* rowperm,
                       const uint32_t* csr_off, const uint32_t* csr_idx, const double* csr_w,
@@ -841,7 +782,6 @@ static int build_sell(sb_em_ctx* c, SellDev& m, uint32_t n_rows, const uint32_t*
   }
   m.n_block = 0;
   m.long_entries = 0;
-  std::vector<uint64_t> h_targets;
   if (m.n_long > 0) {
     // every long row is reduced independently with a fixed tree, so the list order does
     // not affect results.  Longest first: the first n_block rows (> LWARP entries) take
@@ -864,45 +804,10 @@ static int build_sell(sb_em_ctx* c, SellDev& m, uint32_t n_rows, const uint32_t*
       for (int k = 0; k < 3; ++k) h2[3 * i + k] = h[3 * ord[i] + k];
     SB_CUDA(cudaMemcpyAsync(m.long_rows, h2.data(), h2.size() * 4, cudaMemcpyHostToDevice, st));
     SB_CUDA(cudaStreamSynchronize(st));
-    if (c->balance_long > 0 && n_warps > 0) {
-      // The long rows are dealt to warps / blocks by position in the list; charge their cost (in slice columns,
-      // balance_long = percent of one column per 32 entries) to the owner's share of the slice stream.
-      const uint32_t wpb = EM_THREADS / 32, grid = n_warps / wpb;
-      std::vector<double> extra(n_warps, 0.0);
-      for (uint32_t i = 0; i < m.n_long; ++i) {
-        const double L = (double)(h2[3 * i + 2] - h2[3 * i + 1]);
-        if (i < m.n_block) {
-          const uint32_t b = i % grid;
-          for (uint32_t w = 0; w < wpb; ++w) extra[b * wpb + w] += L / EM_THREADS * c->balance_long / 100.0 + 8.0;
-        } else {
-          extra[(i - m.n_block) % n_warps] += L / 32.0 * c->balance_long / 100.0 + 4.0;
-        }
-      }
-      const double total = (double)ncols + (double)overhead * m.n_slices;
-      double sum_extra = 0.0;
-      for (double e : extra) sum_extra += e;
-      const double T = (total + sum_extra) / n_warps;
-      double sum_share = 0.0;
-      for (uint32_t w = 0; w < n_warps; ++w) sum_share += std::max(0.0, T - extra[w]);
-      h_targets.resize(n_warps);
-      double cum = 0.0;
-      for (uint32_t w = 0; w < n_warps; ++w) {
-        h_targets[w] = (uint64_t)(sum_share > 0.0 ? total * (cum / sum_share) : total * w / n_warps);
-        cum += std::max(0.0, T - extra[w]);
-      }
-    }
   }
-  uint64_t* d_targets = nullptr;
-  if (!h_targets.empty()) {
-    SB_TRY(dev_alloc(&m.targets, (size_t)n_warps));
-    SB_CUDA(cudaMemcpyAsync(m.targets, h_targets.data(), h_targets.size() * 8, cudaMemcpyHostToDevice, st));
-    d_targets = m.targets;
-  }
-  k_warp_ranges<<<nblk(n_warps + 1, 256), 256, 0, st>>>(m.n_slices, m.slice_ptr, overhead, n_warps, d_targets,
-                                                        m.warp_begin);
+  k_warp_ranges<<<nblk(n_warps + 1, 256), 256, 0, st>>>(m.n_slices, m.slice_ptr, overhead, n_warps, m.warp_begin);
   c->launches++;
-  SB_CUDA(cudaStreamSynchronize(st));   // h_targets must outlive the copy
-  return split_tails(c, m, overhead, n_warps);
+  return SB_OK;
 }
 
 static int em_rebalance(sb_em_ctx* c);
@@ -1137,12 +1042,9 @@ extern "C" int sb_em_prepare(sb_em_ctx* c, const sb_em_params* p, sb_em_stats* s
 static Sell sell_view(const SellDev& m) {
   Sell s;
   s.slice_ptr = m.slice_ptr; s.base = m.base; s.len = m.len; s.idx = m.idx; s.w = m.w; s.warp_begin = m.warp_begin;
-  s.home_end = m.home_end;
   s.long_rows = m.long_rows; s.csr_idx = m.csr_idx; s.csr_w = m.csr_w;
-  s.tiles = m.tiles;
-  s.n_rows = m.n_rows; s.n_slices = m.n_slices; s.n_long = m.n_long; s.n_tiles = m.n_tiles;
+  s.n_rows = m.n_rows; s.n_slices = m.n_slices; s.n_long = m.n_long;
   s.n_block = m.n_block;
-  s.keep_pct = 100;
   s.zero = m.zero;
   return s;
 }
@@ -1151,8 +1053,6 @@ static void fill_args(sb_em_ctx* c, EmArgs& A, bool row_space) {
   memset(&A, 0, sizeof(A));
   A.cm = sell_view(c->cm);
   A.tm = sell_view(c->tm);
-  A.cm.keep_pct = (uint32_t)c->keep_cm;
-  A.tm.keep_pct = (uint32_t)c->keep_tm;
   // the bootstrap driver's overrides apply only while it is running (ov_active): the buffers outlive it, and a later
   // optimize on the same context must not see the last replicate's resampled counts (bootstrap overrides)
   const bool ov = c->ov_active;
@@ -1587,42 +1487,28 @@ extern "C" int sb_em_run(sb_em_ctx* c, sb_em_stats* stats) {
 }
 
 // Measured re-balancing (a static split by column count does not predict a warp's phase time, and every warp waits
-// at the two grid barriers for the slowest).  One short instrumented run of the persistent
-// kernel accumulates, per warp, the duration of P1 and P2 and of their SELL parts (em_kernels.cuh: SB_ACC_*); the
-// slice ranges are then re-cut so that   long-row time of the warp (fixed: those rows are dealt by list position)
-// + sum over its slices of (measured time density of the warp that ran the slice x modelled slice cost)
-// is equal for all warps (water-filling).  Deterministic given the measurements; the results of the iteration do not
-// depend on the split (each row's sum is computed by one lane in a fixed order wherever the row lands).
-// `unit` = warps that share one range: 1 (ring kernels: a warp owns its range) or 8 (direct kernel: a block's warps take
-// slices from the block's range dynamically; the block's time is the mean of its warps').
-static int em_recut(sb_em_ctx* c, sb::SellDev& m, uint32_t overhead, const std::vector<unsigned long long>& dbg_w,
-                    int slot_total, int slot_sell, uint32_t n_warps_all, uint32_t unit) {
-  const uint32_t n_warps = n_warps_all / unit;        // ranges
+// at the two grid barriers for the slowest).  One short instrumented run of the persistent kernel accumulates, per
+// warp, the duration of P1 and P2 and of their home streams (em_kernels.cuh: SB_ACC_*).  Every slice is given the
+// measured time density of the warp that streamed it (damped towards the mean) times its modelled cost, and the
+// ranges are re-cut so that every warp gets total / n_warps of that measured time.  The long rows are not charged to
+// any warp: they are taken from the phase's work queue by whichever warp is free.  Deterministic given the
+// measurements; the results of the iteration do not depend on the split (each row's sum is computed by one lane in a
+// fixed order wherever the row lands).
+static int em_recut(sb::SellDev& m, uint32_t overhead, const std::vector<unsigned long long>& dbg, int slot_total,
+                    int slot_sell, uint32_t n_warps) {
   if (m.n_slices == 0 || n_warps == 0) return SB_OK;
-  std::vector<uint32_t> sp((size_t)m.n_slices + 1), wb_all((size_t)n_warps_all + 1), wb((size_t)n_warps + 1);
-  std::vector<uint32_t> home_all((size_t)n_warps_all);
+  std::vector<uint32_t> sp((size_t)m.n_slices + 1), wb((size_t)n_warps + 1);
   SB_CUDA(cudaMemcpy(sp.data(), m.slice_ptr, sp.size() * 4, cudaMemcpyDeviceToHost));
-  SB_CUDA(cudaMemcpy(wb_all.data(), m.warp_begin, wb_all.size() * 4, cudaMemcpyDeviceToHost));
-  SB_CUDA(cudaMemcpy(home_all.data(), m.home_end, home_all.size() * 4, cudaMemcpyDeviceToHost));
-  std::vector<unsigned long long> dbg((size_t)n_warps * DBG_SLOTS, 0ull);
-  for (uint32_t r = 0; r <= n_warps; ++r) wb[r] = wb_all[(size_t)r * unit];
-  for (uint32_t r = 0; r < n_warps; ++r)
-    for (uint32_t k = 0; k < DBG_SLOTS; ++k) {
-      unsigned long long a = 0;
-      for (uint32_t u = 0; u < unit; ++u) a += dbg_w[((size_t)r * unit + u) * DBG_SLOTS + k];
-      dbg[(size_t)r * DBG_SLOTS + k] = a / unit;
-    }
+  SB_CUDA(cudaMemcpy(wb.data(), m.warp_begin, wb.size() * 4, cudaMemcpyDeviceToHost));
   auto cost = [&](uint32_t s) { return slice_cost(sp, s, overhead); };
-  std::vector<double> fixed(n_warps), dens(n_warps, 0.0);
+  std::vector<double> dens(n_warps, 0.0);
   double sell_total = 0.0, dens_sum = 0.0, work_sum = 0.0;
   for (uint32_t w = 0; w < n_warps; ++w) {
-    // the SELL tap fires at the end of the home stream: the density is home-part time over home-part work
+    // the SELL tap fires at the end of the home stream: the density is home-stream time over the range's work
     const double T = (double)dbg[(size_t)w * DBG_SLOTS + slot_total];
     const double Ts = std::min(T, (double)dbg[(size_t)w * DBG_SLOTS + slot_sell]);
     double W = 0.0;
-    for (uint32_t u = 0; u < unit; ++u)
-      for (uint32_t s = wb_all[(size_t)w * unit + u]; s < home_all[(size_t)w * unit + u]; ++s) W += cost(s);
-    fixed[w] = 0.0 * (T - Ts);   // the long rows are taken from a global queue: every warp's tail is filled, nothing is fixed
+    for (uint32_t s = wb[w]; s < wb[w + 1]; ++s) W += cost(s);
     if (W > 0.0) { dens[w] = Ts / W; dens_sum += Ts; work_sum += W; }
     sell_total += Ts;
   }
@@ -1639,32 +1525,16 @@ static int em_recut(sb_em_ctx* c, sb::SellDev& m, uint32_t overhead, const std::
     }
   }
   const double total = F[m.n_slices];
-  // level L with sum_w max(0, L - fixed_w) = total
-  double lo = 0.0, hi = total;
-  for (double f : fixed) hi = std::max(hi, f + total);
-  for (int it = 0; it < 100; ++it) {
-    const double L = 0.5 * (lo + hi);
-    double acc = 0.0;
-    for (double f : fixed) acc += std::max(0.0, L - f);
-    if (acc < total) lo = L; else hi = L;
-  }
-  const double L = hi;
   std::vector<uint32_t> nb((size_t)n_warps + 1);
-  double cum = 0.0;
-  uint32_t s = 0;
-  for (uint32_t w = 0; w < n_warps; ++w) {
-    nb[w] = s;
-    cum += std::max(0.0, L - fixed[w]);
-    while (s < m.n_slices && 0.5 * (F[s] + F[s + 1]) < cum) ++s;   // a slice goes to the warp that holds its midpoint
-  }
-  nb[n_warps] = m.n_slices;
   nb[0] = 0;
-  std::vector<uint32_t> nb_all((size_t)n_warps_all + 1);
-  for (uint32_t r = 0; r < n_warps; ++r)
-    for (uint32_t u = 0; u < unit; ++u)    // inside a unit the cut points only matter to the ring kernels: even split
-      nb_all[(size_t)r * unit + u] = nb[r] + (uint32_t)(((uint64_t)(nb[r + 1] - nb[r]) * u) / unit);
-  nb_all[n_warps_all] = m.n_slices;
-  SB_CUDA(cudaMemcpy(m.warp_begin, nb_all.data(), nb_all.size() * 4, cudaMemcpyHostToDevice));
+  nb[n_warps] = m.n_slices;
+  uint32_t s = 0;
+  for (uint32_t w = 1; w < n_warps; ++w) {
+    const double level = total * w / n_warps;
+    while (s < m.n_slices && 0.5 * (F[s] + F[s + 1]) < level) ++s;   // a slice goes to the warp that holds its midpoint
+    nb[w] = s;
+  }
+  SB_CUDA(cudaMemcpy(m.warp_begin, nb.data(), nb.size() * 4, cudaMemcpyHostToDevice));
   return SB_OK;
 }
 
@@ -1683,12 +1553,9 @@ static int em_rebalance(sb_em_ctx* c) {
   if (rc != SB_OK) return rc;
   std::vector<unsigned long long> dbg((size_t)n_warps * DBG_SLOTS);
   SB_CUDA(cudaMemcpy(dbg.data(), c->d_dbg, dbg.size() * 8, cudaMemcpyDeviceToHost));
-  const uint32_t unit = 1u;
   const uint32_t ovh_tm = (uint32_t)(c->params.use_vbem ? c->ovh_p2 : c->ovh_p1);
-  SB_TRY(em_recut(c, c->cm, (uint32_t)c->ovh_p1, dbg, 0, 3, n_warps, unit));
-  SB_TRY(em_recut(c, c->tm, ovh_tm, dbg, 1, 4, n_warps, unit));
-  SB_TRY(split_tails(c, c->cm, (uint32_t)c->ovh_p1, n_warps));
-  SB_TRY(split_tails(c, c->tm, ovh_tm, n_warps));
+  SB_TRY(em_recut(c->cm, (uint32_t)c->ovh_p1, dbg, 0, 3, n_warps));
+  SB_TRY(em_recut(c->tm, ovh_tm, dbg, 1, 4, n_warps));
   return SB_OK;
 }
 

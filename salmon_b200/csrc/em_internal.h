@@ -22,12 +22,7 @@ struct SellDev {
   uint16_t* idx = nullptr;
   double* w = nullptr;
   uint32_t* warp_begin = nullptr;
-  uint32_t* home_end = nullptr;       // per warp: end of the home part of its range (the rest is tail tiles)
   uint32_t* long_rows = nullptr;
-  uint4* tiles = nullptr;             // tail tiles: (first slice, end slice, first column, end column)
-  uint32_t n_tiles = 0;
-  uint64_t home_cols = 0, tail_cols = 0;   // SELL columns in the warps' home parts / in tail tiles
-  uint64_t* targets = nullptr;   // optional per-warp cumulative work targets (balance_long)
   const uint32_t* csr_idx = nullptr;  // not owned
   const double* csr_w = nullptr;      // not owned
 };
@@ -47,19 +42,11 @@ struct sb_em_ctx {
   int config = 1;         // kernel configuration (ring chunk x depth x resident blocks), see kernel_set(); 8x4 b2 is the fastest on H100
   int rebalance = 1;      // rounds of measured re-cutting of the warp ranges at prepare (0 = column-count model only)
   int rebalance_iters = 8;
-  // % of each warp range's modelled work cut off as tail tiles that any warp takes from the phase's work queue, and
-  // the least columns of a tile.  0 = static ranges: on H100 every share measured slower (DESIGN.md section 3.3), because
-  // a tile is reduced from global memory with one dependent index load per group, where the ring path reads shared memory
-  int tail_pct = 0, tail_tile_cols = 16;
   int occ = 0;
   int ovh_p1 = 3, ovh_p2 = 12;
   int lmax = 96;                    // longest row kept on the lane-per-row SELL path
   int sell_group_cm = 1024, sell_group_tm = 1024;   // rows per length-bucketing group (locality window of the gathers)
   int lwarp = 2048;                 // longest row reduced by one warp (longer: one block)
-  int balance_long = 0;             // charge the long rows of a warp / block to its share of the slice stream
-  // % of stream chunks pinned in L2 (evict_last).  0 on H100: the ~67 MB of the two layouts at configs[1] size are
-  // well beyond its 50 MB L2, and pinning any share of them measured slower (DESIGN.md section 3.4)
-  int keep_cm = 0, keep_tm = 0;
 
   // problem
   uint64_t C = 0, nnz = 0;

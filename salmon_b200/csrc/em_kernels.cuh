@@ -15,15 +15,13 @@
 // warp owns a slice: lane = row, each lane accumulates its row sequentially in label order.
 // A slice is exactly as wide as its longest row; an entry is a 16-bit index relative to the
 // slice's base index + an 8-byte weight, 10 bytes (run_phase has the column order).  A slice
-// whose indices span more than 16 bits hands its rows to the long-row path.  Slices are dealt to warps in contiguous ranges cut at prepare time -- first by a column
-// count model, then re-cut from MEASURED per-warp phase times (em.cu: rebalance).  Optionally the last tail_pct % of each
-// range's modelled work is cut off as TAIL TILES (em.cu: split_tails), which go on the phase's work queue after the
-// long rows (off by default: a tile reduced from global memory measured slower than the ring path).
-// Rows longer than LMAX are reduced by a warp / a whole block from their CSR copy.
+// whose indices span more than 16 bits hands its rows to the long-row path.  Slices are dealt to warps in contiguous
+// ranges cut at prepare time -- first by a column count model, then re-cut from MEASURED per-warp phase times (em.cu:
+// rebalance).  Rows longer than LMAX are reduced by a warp / a whole block from their CSR copy.
 //
 // Design points (a warp's time goes to waiting at the grid barriers, L2 gather latency and dependent FP64 chains):
-//   * a warp streams its home range through its ring, then takes long rows (and tail tiles) from one queue until it
-//     is empty.  Every SELL row is summed by one lane in label order, wherever it is reduced;
+//   * a warp streams its slice range through its ring, then takes long rows from the phase's work queue until it is
+//     empty.  Every SELL row is summed by one lane in label order;
 //   * inside a slice the gathers of two groups of 4 columns are issued before either is consumed, and the epilogue
 //     operands of slice s+1 are loaded while slice s is reduced (gathers are not pipelined across slices);
 //   * the VBEM epilogue is one branch-light function (em_math.h) instead of a Boost-style
@@ -60,17 +58,13 @@ struct Sell {
   const uint16_t* len;         // [n_rows] entries per row (LEN_LONG: long path)
   const uint16_t* idx;         // [n_cols*32] gather index - base of the slice (IDX_PAD: padding)
   const double* w;             // [n_cols*32]
-  const uint32_t* warp_begin;  // [n_warps+1] slice range per warp
-  const uint32_t* home_end;    // [n_warps] end of the warp's home part, streamed through its ring; the rest of its
-                               // range is tail tiles
+  const uint32_t* warp_begin;  // [n_warps+1] slice range per warp, streamed through its ring
   // long rows: (row, first entry, end entry) triples into csr_idx / csr_w
   const uint32_t* long_rows;   // [3*n_long]
   const uint32_t* csr_idx;
   const double* csr_w;
-  const uint4* tiles;          // [n_tiles] tail tiles: (first slice, end slice, first column, end column)
-  uint32_t n_rows, n_slices, n_long, n_tiles;
+  uint32_t n_rows, n_slices, n_long;
   uint32_t n_block;            // the first n_block long rows (longest first) take the block path
-  uint32_t keep_pct;           // % of stream chunks loaded with L2 evict_last (rest evict_first)
   uint32_t zero;               // gather slot that always holds 0.0 (what padding entries read)
 };
 
@@ -96,7 +90,7 @@ struct EmArgs {
   uint32_t* out;                // [0]=iters [1]=converged [2]=maxrel slot
   unsigned long long* dbg;      // optional [n_warps*DBG_SLOTS] phase timestamps (ns) of iteration dbg_it
   uint32_t dbg_it;
-  unsigned int* lq;             // [2] work queues (long rows, then tail tiles) of the persistent kernels (P1, P2)
+  unsigned int* lq;             // [2] long-row work queues of the persistent kernels (P1, P2)
   // multi-GPU, fused exchange over peer memory (k_em_persistent_mgpu): every rank owns one exchange block (layout:
   // XchgLayout) mapped into every peer (CUDA IPC, NVLink P2P)
   unsigned char* const* peers;  // [nranks] base pointers of the exchange blocks (peers[rank] = own)
@@ -179,7 +173,7 @@ struct WarpCtx {
   uint64_t* bars;        // [RING]
   uint32_t phase_bits;   // mbarrier parity per stage
   double* scratch;       // block scratch (40 doubles)
-  uint64_t pol_keep, pol_stream;   // L2 eviction policies of the bulk copies
+  uint64_t pol_stream;   // L2 eviction policy of the bulk copies (evict_first: the layouts exceed the L2)
   unsigned long long* dbg;  // optional: the warp's timeline row (end of the home stream, queue items taken)
   unsigned long long* dbg_acc;   // optional: accumulates (end of the SELL part - t0)
   unsigned long long t0;
@@ -195,7 +189,6 @@ __device__ __forceinline__ void warp_setup(WarpCtx<CH, RING>& W, unsigned char* 
   W.dbg = nullptr;
   W.dbg_acc = nullptr;
   W.t0 = 0;
-  W.pol_keep = l2_policy_evict_last();
   W.pol_stream = l2_policy_evict_first();
   if ((threadIdx.x & 31u) == 0) {
 #pragma unroll
@@ -273,7 +266,7 @@ struct WarpRange {
 __device__ __forceinline__ WarpRange load_range(const Sell& S, uint32_t gwarp) {
   WarpRange r;
   r.s0 = __ldg(&S.warp_begin[gwarp]);
-  r.s1 = __ldg(&S.home_end[gwarp]);
+  r.s1 = __ldg(&S.warp_begin[gwarp + 1]);
   r.cbeg = __ldg(&S.slice_ptr[r.s0]);
   r.cend = __ldg(&S.slice_ptr[r.s1]);
   return r;
@@ -284,13 +277,9 @@ __device__ __forceinline__ void ring_issue(const Sell& S, WarpCtx<CH, RING>& W, 
     const uint32_t c = R.cbeg + k * CH;
     const uint32_t cols = min((uint32_t)CH, R.cend - c);
     const int st = k % RING;
-    // The two layouts together exceed what the L2 keeps under a cyclic sweep; pin a fixed
-    // pseudo-random subset of chunks (evict_last) and let the rest stream (evict_first).
-    const bool keep = ((((c / CH) * 2654435761u) >> 24) * 100u >> 8) < S.keep_pct;
-    const uint64_t pol = keep ? W.pol_keep : W.pol_stream;
     mbar_arrive_expect_tx(&W.bars[st], cols * 320u);
-    bulk_g2s_hint(W.ring->w[st], S.w + (size_t)c * 32u, cols * 256u, &W.bars[st], pol);
-    bulk_g2s_hint(W.ring->idx[st], S.idx + (size_t)c * 32u, cols * 64u, &W.bars[st], pol);
+    bulk_g2s_hint(W.ring->w[st], S.w + (size_t)c * 32u, cols * 256u, &W.bars[st], W.pol_stream);
+    bulk_g2s_hint(W.ring->idx[st], S.idx + (size_t)c * 32u, cols * 64u, &W.bars[st], W.pol_stream);
   }
 }
 // fill the ring with the first chunks of a phase.  The matrices are read-only, so this
@@ -312,17 +301,17 @@ __device__ __forceinline__ void ring_drain(WarpCtx<CH, RING>& W, const WarpRange
     if ((uint32_t)k < nchunks) mbar_wait(&W.bars[k], (W.phase_bits >> k) & 1u);
 }
 
-// Where sell_rows reads the entries of column c, counted from the first column of the slices it reduces.  A slice of
+// Where sell_rows reads the entries of column c, counted from the first column of the warp's range.  A slice of
 // width W = its longest row has W / 4 GROUPS of 4 columns and then W % 4 remainder columns.  Inside a group the layout
 // is lane-major,
 //   idx[(group * 32 + lane) * 4 + j],  w[(group * 32 + lane) * 4 + j]        j = 0..3,
 // so a lane reads its four indices with ONE 8-byte load and its four weights with two 16-byte loads and issues the
 // four gathers together; a remainder column is plain column-major (idx[col * 32 + lane]).
 //
-// RingCols: a warp's home range, streamed through its TMA ring.  The ring is a circular buffer of CH * RING columns:
-// column c sits at ring column c % (CH * RING), so a group that straddles two chunks is read in place (each lane's four
-// entries are in one chunk: a chunk boundary falls on a multiple of 32 entries) and a chunk is handed back once the
-// stream has passed its last column.
+// The range streams through the warp's TMA ring, a circular buffer of CH * RING columns: column c sits at ring column
+// c % (CH * RING), so a group that straddles two chunks is read in place (each lane's four entries are in one chunk: a
+// chunk boundary falls on a multiple of 32 entries) and a chunk is handed back once the stream has passed its last
+// column.
 template <int CH, int RING>
 struct RingCols {
   static constexpr uint32_t RC = (uint32_t)(CH * RING);   // ring capacity in columns
@@ -357,32 +346,15 @@ struct RingCols {
   __device__ __forceinline__ uint32_t idx1(uint32_t c) const { return (&W.ring->idx[0][0])[(c % RC) * 32u + lane]; }
   __device__ __forceinline__ double w1(uint32_t c) const { return (&W.ring->w[0][0])[(c % RC) * 32u + lane]; }
 };
-// GlobalCols: a tail tile, read straight from the layout in global memory
-struct GlobalCols {
-  const uint16_t* idx;   // the tile's first column
-  const double* w;
-  uint32_t lane;
-  __device__ __forceinline__ void need(uint32_t, uint32_t) const {}
-  __device__ __forceinline__ uint2 idx4(uint32_t c) const {
-    return __ldg(reinterpret_cast<const uint2*>(idx + c * 32u + lane * 4u));
-  }
-  __device__ __forceinline__ double2 w4(uint32_t c, uint32_t j) const {
-    return __ldg(reinterpret_cast<const double2*>(w + c * 32u + lane * 4u + j));
-  }
-  __device__ __forceinline__ uint32_t idx1(uint32_t c) const { return __ldg(idx + c * 32u + lane); }
-  __device__ __forceinline__ double w1(uint32_t c) const { return __ldg(w + c * 32u + lane); }
-};
-
-// The rows of slices [s0, s1), whose columns are [cbeg, cend) of the layout, read through `cols`.  Every row is summed
-// by one lane in label order -- pairs of groups (8 gathers in flight), then a single group, then the remainder columns
-// -- and finished (row_finish) with operands loaded one slice ahead.  The ring path and the tail-tile path both call
-// this, so a row's sum does not depend on which path reduced it.  The remainder is the same for the 32 lanes, so it is
-// a warp-uniform branch, not a per-lane predicate.  Padding entries (a row shorter than its slice) have weight 0 and
-// gather a slot that always holds 0.0, so a row's sum is its label-order sum.
-template <int PHASE, bool VBEM, class Cols, class Deliver>
-__device__ __forceinline__ void sell_rows(const EmArgs& A, const Sell& S, Cols& cols, uint32_t s0, uint32_t s1,
-                                          uint32_t cbeg, uint32_t cend, double logNorm, double bias, P2Acc& pa,
-                                          Deliver&& deliver) {
+// The rows of slices [s0, s1), whose columns are [cbeg, cend) of the layout, read through the ring `cols`.  Every row
+// is summed by one lane in label order -- pairs of groups (8 gathers in flight), then a single group, then the
+// remainder columns -- and finished (row_finish) with operands loaded one slice ahead.  The remainder is the same for
+// the 32 lanes, so it is a warp-uniform branch, not a per-lane predicate.  Padding entries (a row shorter than its
+// slice) have weight 0 and gather a slot that always holds 0.0, so a row's sum is its label-order sum.
+template <int PHASE, bool VBEM, int CH, int RING, class Deliver>
+__device__ __forceinline__ void sell_rows(const EmArgs& A, const Sell& S, RingCols<CH, RING>& cols, uint32_t s0,
+                                          uint32_t s1, uint32_t cbeg, uint32_t cend, double logNorm, double bias,
+                                          P2Acc& pa, Deliver&& deliver) {
   // theta / scale are rewritten by other blocks inside the persistent kernel: plain
   // coherent loads only, never ld.global.nc.
   const double* gsrc = (PHASE == 1) ? A.theta : A.scale;
@@ -471,9 +443,8 @@ struct Nothing {
 };
 
 // One phase of a warp: its home range through the ring, then `after_home` (the ring is idle from there on: the caller
-// hands it to the next phase's home range), then the block-path rows, then the phase's work queue.  Queue items
-// [0, n_mid) are the long rows (LMAX < len <= LWARP), longest first; items [n_mid, n_mid + n_tiles) are the tail
-// tiles.  Big items first, small ones fill the end.
+// hands it to the next phase's home range), then the block-path rows, then the phase's work queue: items [0, n_mid)
+// are the warp-path long rows (LMAX < len <= LWARP), longest first, so the short ones fill the end of the phase.
 template <int PHASE, int CH, int RING, bool VBEM, bool DYNQ, class AfterHome, class Deliver>
 __device__ __forceinline__ void run_phase(const EmArgs& A, WarpCtx<CH, RING>& W, const WarpRange& R,
                                           uint32_t bid, uint32_t nblk, double logNorm, double bias,
@@ -531,7 +502,7 @@ __device__ __forceinline__ void run_phase(const EmArgs& A, WarpCtx<CH, RING>& W,
   {
     const uint32_t gw = bid * EM_WARPS + (threadIdx.x >> 5);
     const uint32_t nw = nblk * EM_WARPS;
-    const uint32_t n_mid = S.n_long - S.n_block, n_items = n_mid + S.n_tiles;
+    const uint32_t n_mid = S.n_long - S.n_block;
     unsigned int* queue = A.lq + ((PHASE == 1) ? 0 : 1);
     // lane k keeps the sum of the k-th long row this warp reduced; the epilogues (digamma, exp)
     // then run lane-parallel, 32 rows at a time.
@@ -551,89 +522,69 @@ __device__ __forceinline__ void run_phase(const EmArgs& A, WarpCtx<CH, RING>& W,
       if (lane == 0) q = atomicAdd(queue, 1u);
       return q;               // lane 0's value is broadcast when it is consumed
     };
-    // an item: (row, first entry, end entry) of a long row, or (first slice, end slice, first column, end column) of a
-    // tail tile
-    auto item = [&](uint32_t q) {
-      uint4 d = make_uint4(0u, 0u, 0u, 0u);
-      if (q < n_mid) {
-        const uint32_t li = S.n_block + q;
-        d.x = __ldg(&S.long_rows[3 * li]);
-        d.y = __ldg(&S.long_rows[3 * li + 1]);
-        d.z = __ldg(&S.long_rows[3 * li + 2]);
-      } else if (q < n_items) {
-        d = __ldg(&S.tiles[q - n_mid]);
-      }
-      return d;
-    };
     uint32_t q_next;
-    if (DYNQ) q_next = n_items ? claim() : 0u; else q_next = gw;
+    if (DYNQ) q_next = n_mid ? claim() : 0u; else q_next = gw;
     // timeline: what this warp took from the queue (slots zeroed when the timeline is armed)
-    unsigned long long* const qs = (dbg && lane == 0) ? dbg + (PHASE == 1 ? 9 : 12) : nullptr;
+    unsigned long long* const qs = (dbg && lane == 0) ? dbg + (PHASE == 1 ? 9 : 11) : nullptr;
     for (;;) {
       const uint32_t q = DYNQ ? __shfl_sync(0xffffffffu, q_next, 0) : q_next;
-      if (q >= n_items) break;
+      if (q >= n_mid) break;
       if (DYNQ) q_next = claim(); else q_next = q + nw;
-      const uint4 d = item(q);
-      if (q < n_mid) {
-        // one warp per row, lanes stride the CSR copy with four independent gathers in flight, fixed shuffle tree.
-        // The CSR loads of step k + 128 are issued before the gathers of step k are consumed.
-        const uint32_t r = d.x, b = d.y, e = d.z;
-        double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
-        uint32_t k = b + lane;
-        uint32_t i0 = 0u, i1 = 0u, i2 = 0u, i3 = 0u;
-        double w0 = 0.0, w1 = 0.0, w2 = 0.0, w3 = 0.0;
-        if (k + 96 < e) {
-          i0 = __ldg(&S.csr_idx[k]); i1 = __ldg(&S.csr_idx[k + 32]);
-          i2 = __ldg(&S.csr_idx[k + 64]); i3 = __ldg(&S.csr_idx[k + 96]);
-          w0 = __ldg(&S.csr_w[k]); w1 = __ldg(&S.csr_w[k + 32]);
-          w2 = __ldg(&S.csr_w[k + 64]); w3 = __ldg(&S.csr_w[k + 96]);
-        }
-        for (; k + 96 < e; k += 128) {
-          const double g0 = gsrc[i0], g1 = gsrc[i1], g2 = gsrc[i2], g3 = gsrc[i3];
-          const double x0 = w0, x1 = w1, x2 = w2, x3 = w3;
-          // no branch around the next step's loads (a last step reloads its own entries), so that they can be issued
-          // ahead of this step's FMAs
-          const uint32_t kn = (k + 224 < e) ? k + 128 : k;
-          i0 = __ldg(&S.csr_idx[kn]); i1 = __ldg(&S.csr_idx[kn + 32]);
-          i2 = __ldg(&S.csr_idx[kn + 64]); i3 = __ldg(&S.csr_idx[kn + 96]);
-          w0 = __ldg(&S.csr_w[kn]); w1 = __ldg(&S.csr_w[kn + 32]);
-          w2 = __ldg(&S.csr_w[kn + 64]); w3 = __ldg(&S.csr_w[kn + 96]);
-          double v0 = g0 * x0, v1 = g1 * x1;
-          double v2 = g2 * x2, v3 = g3 * x3;
-          if (GUARD) {
-            if (isnan(v0)) v0 = 0.0;
-            if (isnan(v1)) v1 = 0.0;
-            if (isnan(v2)) v2 = 0.0;
-            if (isnan(v3)) v3 = 0.0;
-          }
-          a0 += v0; a1 += v1; a2 += v2; a3 += v3;
-        }
-        {
-          // tail: up to three more strides, issued together
-          const uint32_t j0 = (k < e) ? __ldg(&S.csr_idx[k]) : 0u;
-          const uint32_t j1 = (k + 32 < e) ? __ldg(&S.csr_idx[k + 32]) : 0u;
-          const uint32_t j2 = (k + 64 < e) ? __ldg(&S.csr_idx[k + 64]) : 0u;
-          double v0 = (k < e) ? gsrc[j0] * __ldg(&S.csr_w[k]) : 0.0;
-          double v1 = (k + 32 < e) ? gsrc[j1] * __ldg(&S.csr_w[k + 32]) : 0.0;
-          double v2 = (k + 64 < e) ? gsrc[j2] * __ldg(&S.csr_w[k + 64]) : 0.0;
-          if (GUARD) {
-            if (isnan(v0)) v0 = 0.0;
-            if (isnan(v1)) v1 = 0.0;
-            if (isnan(v2)) v2 = 0.0;
-          }
-          a0 += v0; a1 += v1; a2 += v2;
-        }
-        const double acc = warp_sum((a0 + a1) + (a2 + a3));
-        if (lane == cnt) { myacc = acc; myrow = r; }
-        if (++cnt == 32) flush();
-        if (qs) { qs[0] += (1ull << 32) | (e - b); qs[2] = max(qs[2], (unsigned long long)(e - b)); }
-      } else {
-        if (d.w > d.z) {
-          GlobalCols gc{S.idx + (size_t)d.z * 32u, S.w + (size_t)d.z * 32u, lane};
-          sell_rows<PHASE, VBEM>(A, S, gc, d.x, d.y, d.z, d.w, logNorm, bias, pa, deliver);
-        }
-        if (qs) qs[1] += (1ull << 32) | (d.w - d.z);
+      // one warp per row, lanes stride the CSR copy with four independent gathers in flight, fixed shuffle tree.
+      // The CSR loads of step k + 128 are issued before the gathers of step k are consumed.
+      const uint32_t li = S.n_block + q;
+      const uint32_t r = __ldg(&S.long_rows[3 * li]);
+      const uint32_t b = __ldg(&S.long_rows[3 * li + 1]);
+      const uint32_t e = __ldg(&S.long_rows[3 * li + 2]);
+      double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
+      uint32_t k = b + lane;
+      uint32_t i0 = 0u, i1 = 0u, i2 = 0u, i3 = 0u;
+      double w0 = 0.0, w1 = 0.0, w2 = 0.0, w3 = 0.0;
+      if (k + 96 < e) {
+        i0 = __ldg(&S.csr_idx[k]); i1 = __ldg(&S.csr_idx[k + 32]);
+        i2 = __ldg(&S.csr_idx[k + 64]); i3 = __ldg(&S.csr_idx[k + 96]);
+        w0 = __ldg(&S.csr_w[k]); w1 = __ldg(&S.csr_w[k + 32]);
+        w2 = __ldg(&S.csr_w[k + 64]); w3 = __ldg(&S.csr_w[k + 96]);
       }
+      for (; k + 96 < e; k += 128) {
+        const double g0 = gsrc[i0], g1 = gsrc[i1], g2 = gsrc[i2], g3 = gsrc[i3];
+        const double x0 = w0, x1 = w1, x2 = w2, x3 = w3;
+        // no branch around the next step's loads (a last step reloads its own entries), so that they can be issued
+        // ahead of this step's FMAs
+        const uint32_t kn = (k + 224 < e) ? k + 128 : k;
+        i0 = __ldg(&S.csr_idx[kn]); i1 = __ldg(&S.csr_idx[kn + 32]);
+        i2 = __ldg(&S.csr_idx[kn + 64]); i3 = __ldg(&S.csr_idx[kn + 96]);
+        w0 = __ldg(&S.csr_w[kn]); w1 = __ldg(&S.csr_w[kn + 32]);
+        w2 = __ldg(&S.csr_w[kn + 64]); w3 = __ldg(&S.csr_w[kn + 96]);
+        double v0 = g0 * x0, v1 = g1 * x1;
+        double v2 = g2 * x2, v3 = g3 * x3;
+        if (GUARD) {
+          if (isnan(v0)) v0 = 0.0;
+          if (isnan(v1)) v1 = 0.0;
+          if (isnan(v2)) v2 = 0.0;
+          if (isnan(v3)) v3 = 0.0;
+        }
+        a0 += v0; a1 += v1; a2 += v2; a3 += v3;
+      }
+      {
+        // tail: up to three more strides, issued together
+        const uint32_t j0 = (k < e) ? __ldg(&S.csr_idx[k]) : 0u;
+        const uint32_t j1 = (k + 32 < e) ? __ldg(&S.csr_idx[k + 32]) : 0u;
+        const uint32_t j2 = (k + 64 < e) ? __ldg(&S.csr_idx[k + 64]) : 0u;
+        double v0 = (k < e) ? gsrc[j0] * __ldg(&S.csr_w[k]) : 0.0;
+        double v1 = (k + 32 < e) ? gsrc[j1] * __ldg(&S.csr_w[k + 32]) : 0.0;
+        double v2 = (k + 64 < e) ? gsrc[j2] * __ldg(&S.csr_w[k + 64]) : 0.0;
+        if (GUARD) {
+          if (isnan(v0)) v0 = 0.0;
+          if (isnan(v1)) v1 = 0.0;
+          if (isnan(v2)) v2 = 0.0;
+        }
+        a0 += v0; a1 += v1; a2 += v2;
+      }
+      const double acc = warp_sum((a0 + a1) + (a2 + a3));
+      if (lane == cnt) { myacc = acc; myrow = r; }
+      if (++cnt == 32) flush();
+      if (qs) { qs[0] += (1ull << 32) | (e - b); qs[1] = max(qs[1], (unsigned long long)(e - b)); }
     }
     flush();
   }
@@ -684,8 +635,8 @@ __device__ __forceinline__ void p2_finish(const EmArgs& A, double* scratch, P2Ac
 // iterations >= 1 of a run (dbg_it = DBG_ACCUMULATE; slot 0 = P1, slot 1 = P2, slot 2 = iterations) -- the input of
 // the measured re-balancing in em.cu (slots 3 / 4: the home stream of P1 / P2 alone).  One iteration's row of the
 // persistent kernel: 0 P1 start, 1 P1 end, 2 end of barrier 1, 3 P2 start, 4 P2 end, 5 reduction end, 6 end of
-// barrier 2, 7 / 8 end of the P2 / P1 home stream, 9-11 / 12-14 what the warp took from the P1 / P2 queue:
-// (long rows << 32 | their entries), (tail tiles << 32 | their columns), longest row taken (run_phase)
+// barrier 2, 7 / 8 end of the P2 / P1 home stream, 9-10 / 11-12 what the warp took from the P1 / P2 queue:
+// (long rows << 32 | their entries), longest row taken (run_phase)
 #define SB_DBG(slot)                                                        \
   if (A.dbg && it == A.dbg_it && (threadIdx.x & 31u) == 0) A.dbg[(size_t)gwarp * DBG_SLOTS + (slot)] = gtime_ns();
 #define SB_ACC_BEGIN(var, sell_slot) \

@@ -1,5 +1,5 @@
 """Per-warp phase timeline of one iteration of the persistent EM kernel (dev helper).
-usage: timeline_em.py [C] [key=value ...]      (sb_em_set_option keys, e.g. tail_pct=0)"""
+usage: timeline_em.py [C] [key=value ...]      (sb_em_set_option keys, e.g. rebalance=0)"""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -17,7 +17,6 @@ ctx.run()
 nw = ctx.arm_timeline(40)
 r = ctx.run()
 t = ctx.read_timeline(nw).astype(np.int64)
-queue_taps = t.shape[1] >= 15      # builds with tail tiles also record the P1 home end and the queue items per warp
 t0 = t[:, 0].min()
 names = ["P1 start", "P1 end", "bar1 end", "P2 start", "P2 end", "reduce end", "bar2 end"]
 sizes = (eq.off[1:] - eq.off[:-1]).astype(np.int64)
@@ -30,9 +29,6 @@ print("stream per iteration: %.2f MB (class-major %.2f, transcript-major %.2f; S
           sb / 1e6, ctx.info("stream_bytes_cm") / 1e6, ctx.info("stream_bytes_tm") / 1e6, ctx.info("sell_cols_cm"),
           ctx.info("sell_cols_tm"), ctx.info("long_entries_cm"), ctx.info("long_entries_tm"), ctx.info("fallback_rows_cm"),
           ctx.info("fallback_rows_tm"), sb / (r.loop_kernel_ms / 60 * 1e-3) / 1e9))
-if queue_taps:
-    print("tail tiles %d / %d, tail columns %d / %d" % (ctx.info("tail_tiles_cm"), ctx.info("tail_tiles_tm"),
-                                                       ctx.info("tail_cols_cm"), ctx.info("tail_cols_tm")))
 for i, n in enumerate(names):
     col = t[:, i] - t0
     print(f"{n:11s} min {col.min()/1e3:8.2f}  p50 {np.median(col)/1e3:8.2f}  p90 {np.percentile(col,90)/1e3:8.2f}  max {col.max()/1e3:8.2f} us")
@@ -48,15 +44,13 @@ for ph, (c_end, c_start) in (("P1", (1, 0)), ("P2", (4, 3))):
 
 
 def items(row, base):
-    lr, tl = int(row[base]), int(row[base + 1])
-    return "long rows %3d (%6d entries, longest %4d)  tiles %3d (%4d cols)" % (lr >> 32, lr & 0xFFFFFFFF, int(row[base + 2]),
-                                                                            tl >> 32, tl & 0xFFFFFFFF)
+    lr = int(row[base])
+    return "long rows %3d (%6d entries, longest %4d)" % (lr >> 32, lr & 0xFFFFFFFF, int(row[base + 1]))
 
 
-for ph, (c_start, c_end, c_home, q_base) in (("P1", (0, 1, 8, 9)), ("P2", (3, 4, 7, 12))):
+for ph, (c_start, c_end, c_home, q_base) in (("P1", (0, 1, 8, 9)), ("P2", (3, 4, 7, 11))):
     d = t[:, c_end] - t[:, c_start]
     print("10 slowest %s warps (us from the warp's phase start):" % ph)
     for w in np.argsort(-d)[:10]:
-        home = "%7.2f" % ((t[w, c_home] - t[w, c_start]) / 1e3) if queue_taps or ph == "P2" else "    n/a"
-        q = items(t[w], q_base) if queue_taps else "queue items not recorded by this build"
-        print("  warp %5d  home end %s  phase end %7.2f  %s" % (w, home, d[w] / 1e3, q))
+        home = (t[w, c_home] - t[w, c_start]) / 1e3
+        print("  warp %5d  home end %7.2f  phase end %7.2f  %s" % (w, home, d[w] / 1e3, items(t[w], q_base)))

@@ -298,6 +298,12 @@ typedef struct sb_map_params {
    * anchor's transcript within max_frag_len for the missing mate (infix edit distance) and turn the orphans into the
    * pairs found (rule: DESIGN.md section 11).  Single-end libraries ignore it. */
   int32_t recover_orphans;
+  /* scoring mode of the banded DP (rule: DESIGN.md section 12): 0 = end-to-end (default), 1 = --softclipOverhangs
+   * (read bases hanging over either transcript end are left unaligned and add nothing to the score), 2 = --softclip
+   * (any stretch of the read may be left unaligned at either end: the score is the best local alignment inside the
+   * band; includes 1).  The acceptance threshold stays minScoreFraction * ma * read length.  Other values are refused;
+   * variant 0 of the mapping kernels supports 0 only. */
+  int32_t softclip;
 } sb_map_params;
 /* Only sb_quant_files takes these two: the library type is detected from the first 50 000 fragments that show a
  * strand, as LibraryTypeDetector does (include/salmon/internal/model/LibraryTypeDetector.hpp:34-140): until then every

@@ -83,7 +83,7 @@ class sb_map_params(C.Structure):
         ("seed", C.c_uint64), ("mini_batch", C.c_uint32), ("reserved2", C.c_uint32),
         ("pre_merge_thresh", C.c_double), ("post_merge_thresh", C.c_double), ("orphan_thresh", C.c_double),
         ("allow_dovetail", C.c_int32), ("allow_orphans", C.c_int32), ("lib_type", C.c_int32),
-        ("recover_orphans", C.c_int32),
+        ("recover_orphans", C.c_int32), ("softclip", C.c_int32),
     ]
 
 

@@ -75,7 +75,7 @@ int usage() {
           "  sb_salmon index -t transcripts.fa[.gz] -i index_dir [-k 31] [--gencode] [-d decoys.txt] [--keepDuplicates] [--no-clip]\n"
           "  sb_salmon quant -i index_dir -l IU|ISF|ISR -1 r1.fq[.gz] ... -2 r2.fq[.gz] ... | -l U|SF|SR -r reads.fq[.gz] ...  -o out_dir [--gpus N]\n"
           "                  [-p threads] [--dumpEq] [--dumpEqWeights] [--writeMappings[=FILE] | -z] [--writeQualities] [--writeUnmappedNames]\n"
-          "                  [--recoverOrphans]\n"
+          "                  [--recoverOrphans] [--softclip] [--softclipOverhangs]\n"
           "                  [--numBootstraps N | --numGibbsSamples N] [--thinningFactor 16] [--noGammaDraw] [--useEM] [--vbPrior 0.01]\n"
           "                  [--perNucleotidePrior] [--maxReadOcc 200] [--maxOccsPerHit 1000] [--minScoreFraction 0.65] [--consensusSlack 0.35]\n"
           "                  [--preMergeChainSubThresh 0.75] [--postMergeChainSubThresh 0.9] [--orphanChainSubThresh 0.95] [--allowDovetail]\n"
@@ -269,7 +269,9 @@ int cmd_quant(Args& a) {
     else if (o == "--batch") { if (!num(d)) return usage(); qo.batch = (uint32_t)d; }
     else if (o == "--maxReadLen") { if (!num(d)) return usage(); qo.max_read_len = (uint32_t)d; }
     else if (o == "--seed") { if (!num(d)) return usage(); qo.seed = (uint64_t)d; mp.seed = (uint64_t)d; }
-    else if (o == "--validateMappings" || o == "--softclipOverhangs" || o == "-q" || o == "--quiet") { /* default behaviour / no-op */ }
+    else if (o == "--validateMappings" || o == "-q" || o == "--quiet") { /* default behaviour / no-op */ }
+    else if (o == "--softclipOverhangs") { if (mp.softclip < 1) mp.softclip = 1; }   // --softclip includes it
+    else if (o == "--softclip") mp.softclip = 2;
     else if (o == "--writeMappings" || o == "-z") sam_path = "-";   // (SAM on standard output)
     else if (o.rfind("--writeMappings=", 0) == 0) sam_path = o.substr(16);
     else if (o == "--writeQualities") qo.write_qualities = 1;

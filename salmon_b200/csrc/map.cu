@@ -1061,6 +1061,15 @@ static int dmalloc(T** p, size_t n) {
 }
 static inline unsigned nblk(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
 
+// the three DP kernels of one chunk for scoring mode MODE (Params::softclip); the same launches in every mode
+template <int NWR, int MODE>
+static void launch_dp(const sb_map_ctx* c, cudaStream_t st, const IndexView& ix, const Params& p, uint32_t L,
+                      const uint8_t* dl, const uint8_t* dr, const DpIo& io) {
+  k_dp_classify<NWR, MODE><<<c->n_sm * 3, 256, 0, st>>>(ix, p, c->pr, L, c->fast_ok, io);
+  k_dp_pair<NWR, MODE == 2 ? 2 : 0><<<c->n_sm * (NWR == 4 ? 3 : 2), 256, 0, st>>>(ix, p, c->pr, L, io);
+  k_dp_general<NWR, MODE><<<c->n_sm * 3, 256, 0, st>>>(ix, p, c->pr, dl, dr, L, c->ascii, io);
+}
+
 extern "C" void sb_map_default_params(sb_map_params* q) {
   memset(q, 0, sizeof(*q));
   q->k = 31; q->stride = 4; q->max_occs_per_hit = 1000; q->max_read_occ = 200; q->max_frag_len = 1000;
@@ -1148,6 +1157,10 @@ static inline double wall_s() {
 extern "C" sb_map_ctx* sb_map_create(sb_index* ix, const sb_map_params* q, int device, uint32_t batch_cap,
                                      uint32_t max_read_len) {
   if (!ix || !q) { sb::set_error("null argument"); return nullptr; }
+  if (q->softclip < 0 || q->softclip > 2) {
+    sb::set_error("sb_map_create: unsupported softclip mode %d (0 end-to-end, 1 overhangs, 2 soft-clip)", q->softclip);
+    return nullptr;
+  }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
     cudaGetLastError();
@@ -1174,7 +1187,7 @@ extern "C" sb_map_ctx* sb_map_create(sb_index* ix, const sb_map_params* q, int d
   p.seed = q->seed; p.mini_batch = q->mini_batch ? q->mini_batch : 5000; p.reserved = 0;
   p.pre_merge_thresh = q->pre_merge_thresh; p.post_merge_thresh = q->post_merge_thresh; p.orphan_thresh = q->orphan_thresh;
   p.allow_dovetail = q->allow_dovetail; p.allow_orphans = q->allow_orphans;
-  p.lib_type = q->lib_type; p.recover_orphans = q->recover_orphans ? 1 : 0;
+  p.lib_type = q->lib_type; p.recover_orphans = q->recover_orphans ? 1 : 0; p.softclip = q->softclip;
   if (p.lib_type < 0 || p.lib_type > 5) { sb::set_error("unsupported library type %d (IU, ISF, ISR, U, SF, SR)", p.lib_type); delete c; return nullptr; }
   if (!(p.pre_merge_thresh >= 0 && p.pre_merge_thresh <= 1) || !(p.post_merge_thresh >= 0 && p.post_merge_thresh <= 1) ||
       !(p.orphan_thresh >= 0 && p.orphan_thresh <= 1)) {
@@ -1327,6 +1340,7 @@ extern "C" int sb_map_set_option(sb_map_ctx* c, const char* key, int64_t value) 
   if (!c || !key) { sb::set_error("null argument"); return SB_ERR_INVALID; }
   if (!strcmp(key, "variant")) {
     if (value == 0 && c->p.recover_orphans) { sb::set_error("recover_orphans needs the warp kernels (variant 1)"); return SB_ERR_INVALID; }
+    if (value == 0 && c->p.softclip) { sb::set_error("softclip modes 1 and 2 need the warp kernels (variant 1)"); return SB_ERR_INVALID; }
     c->variant = (int)value;
     return SB_OK;
   }
@@ -1531,16 +1545,20 @@ static int map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, u
         if (npos <= 32) k_seed_chain_w<2, 1><<<c->seed_blocks, SeedCfg<2>::WARPS * 32, 0, st>>>(ix, p, c->pr, cn, L, so);
         else k_seed_chain_w<2, 2><<<c->seed_blocks, SeedCfg<2>::WARPS * 32, 0, st>>>(ix, p, c->pr, cn, L, so);
         SB_CUDA(cudaEventRecord(c->ev_seed[2 * ch + 1], st));
-        k_dp_classify<4><<<c->n_sm * 3, 256, 0, st>>>(ix, p, c->pr, L, c->fast_ok, io);
-        k_dp_pair<4><<<c->n_sm * 3, 256, 0, st>>>(ix, p, c->pr, L, io);
-        k_dp_general<4><<<c->n_sm * 3, 256, 0, st>>>(ix, p, c->pr, dl, dr, L, c->ascii, io);
+        switch (p.softclip) {
+          case 0: launch_dp<4, 0>(c, st, ix, p, L, dl, dr, io); break;
+          case 1: launch_dp<4, 1>(c, st, ix, p, L, dl, dr, io); break;
+          default: launch_dp<4, 2>(c, st, ix, p, L, dl, dr, io); break;
+        }
       } else {
         if (npos <= 32) k_seed_chain_w<4, 1><<<c->seed_blocks, SeedCfg<4>::WARPS * 32, 0, st>>>(ix, p, c->pr, cn, L, so);
         else k_seed_chain_w<4, 2><<<c->seed_blocks, SeedCfg<4>::WARPS * 32, 0, st>>>(ix, p, c->pr, cn, L, so);
         SB_CUDA(cudaEventRecord(c->ev_seed[2 * ch + 1], st));
-        k_dp_classify<8><<<c->n_sm * 3, 256, 0, st>>>(ix, p, c->pr, L, c->fast_ok, io);
-        k_dp_pair<8><<<c->n_sm * 2, 256, 0, st>>>(ix, p, c->pr, L, io);
-        k_dp_general<8><<<c->n_sm * 3, 256, 0, st>>>(ix, p, c->pr, dl, dr, L, c->ascii, io);
+        switch (p.softclip) {
+          case 0: launch_dp<8, 0>(c, st, ix, p, L, dl, dr, io); break;
+          case 1: launch_dp<8, 1>(c, st, ix, p, L, dl, dr, io); break;
+          default: launch_dp<8, 2>(c, st, ix, p, L, dl, dr, io); break;
+        }
       }
       c->launches += 5;
     }
@@ -1560,7 +1578,11 @@ static int map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, u
         case 3: k_rescue_search<3><<<sb, 128, 0, st>>>(ix, p, c->pr, L, bc.cand_l, bc.cand_r, rb); break;
         default: k_rescue_search<4><<<sb, 128, 0, st>>>(ix, p, c->pr, L, bc.cand_l, bc.cand_r, rb); break;
       }
-      k_rescue_score<<<c->n_sm * 4, 256, 0, st>>>(ix, p, dl, dr, L, c->ascii, bc.cand_l, bc.cand_r, rb);
+      switch (p.softclip) {
+        case 0: k_rescue_score<0><<<c->n_sm * 4, 256, 0, st>>>(ix, p, dl, dr, L, c->ascii, bc.cand_l, bc.cand_r, rb); break;
+        case 1: k_rescue_score<1><<<c->n_sm * 4, 256, 0, st>>>(ix, p, dl, dr, L, c->ascii, bc.cand_l, bc.cand_r, rb); break;
+        default: k_rescue_score<2><<<c->n_sm * 4, 256, 0, st>>>(ix, p, dl, dr, L, c->ascii, bc.cand_l, bc.cand_r, rb); break;
+      }
       k_rescue_commit<<<nblk(cn, 128), 128, 0, st>>>(p, cn, L, bc.n_l, bc.n_r, bc.cand_l, bc.cand_r, bc.score_l, bc.score_r, rb);
       SB_CUDA(cudaEventRecord(c->ev_rescue[2 * ch + 1], st));
       c->launches += 4;

@@ -39,6 +39,7 @@ struct Params {
   int32_t allow_dovetail, allow_orphans;
   int32_t lib_type;                 // expected library format (SB_LIB_*)
   int32_t recover_orphans;          // --recoverOrphans (DESIGN.md §11); 0 = off
+  int32_t softclip;                 // scoring mode (DESIGN.md §12): 0 end-to-end, 1 --softclipOverhangs, 2 --softclip
 };
 
 struct TableEntry {
@@ -435,12 +436,21 @@ SB_HD uint32_t for_each_joint(const Params& p, const Cand* lc, uint32_t nl, cons
 
 // ---- banded affine glocal DP, serial form (host tests; device fallback).  The warp form in
 // map.cu computes the same recurrences with lanes = band cells.
+// Scoring mode p.softclip (DESIGN.md §12):
+//   0  end-to-end: every read base is aligned, cells outside the transcript are dead, the score is the best cell of the
+//      last row;
+//   1  overhangs: in addition a path may start at any row in the cell of reference column 0 (the diagonal predecessor
+//      counts as 0) and end at any row in the cell of column tlen-1 (the bases before / after it score 0);
+//   2  soft-clip: every live cell may start a path (diagonal predecessor floored at 0) and the score is the best live
+//      cell of any row.
 SB_HD int32_t dp_score_serial(const IndexView& ix, const Params& p, const uint8_t* read, uint32_t L,
                               uint32_t ori, uint32_t tid, int32_t diag_c) {
   const int32_t B = (int32_t)p.band, W = 2 * B + 1;
+  const int32_t mode = p.softclip;
   const int64_t tlen = (int64_t)(ix.tx_off[tid + 1] - ix.tx_off[tid]);
   const uint8_t* ref = ix.codes + ix.tx_off[tid];
   int32_t H[64], E[64];
+  int32_t best = NEG_SCORE;   // modes 1 and 2: best end before the last row
   for (int32_t j = 0; j < W; ++j) { H[j] = 0; E[j] = NEG_SCORE; }
   for (uint32_t i = 0; i < L; ++i) {
     const uint8_t c = ori ? read[L - 1 - i] : read[i];
@@ -454,7 +464,9 @@ SB_HD int32_t dp_score_serial(const IndexView& ix, const Params& p, const uint8_
       int32_t h = NEG_SCORE, e = NEG_SCORE, f = NEG_SCORE;
       if (r >= 0 && r < tlen) {
         const int32_t s = (rb < 4 && rb == ref[r]) ? p.ma : p.mp;
-        const int32_t m = H[j] + s;
+        int32_t hd = H[j];
+        if ((mode == 2 || (mode == 1 && r == 0)) && hd < 0) hd = 0;   // a path starts here
+        const int32_t m = hd + s;
         if (j + 1 < W) { const int32_t a = Hup - p.go - p.ge, b = Eup - p.ge; e = a > b ? a : b; }
         if (j > 0) { const int32_t a = Hleft - p.go - p.ge, b = Fprev - p.ge; f = a > b ? a : b; }
         h = m;
@@ -463,13 +475,13 @@ SB_HD int32_t dp_score_serial(const IndexView& ix, const Params& p, const uint8_
         if (h < NEG_SCORE) h = NEG_SCORE;
         if (e < NEG_SCORE) e = NEG_SCORE;
         if (f < NEG_SCORE) f = NEG_SCORE;
+        if ((mode == 2 || (mode == 1 && r == tlen - 1)) && h > best) best = h;   // a path ends here
       }
       (void)Hn_next_diag;
       H[j] = h; E[j] = e;     // lane j of the previous row is no longer needed (lane j-1 used H[j] already)
       Hleft = h; Fprev = f;
     }
   }
-  int32_t best = NEG_SCORE;
   for (int32_t j = 0; j < W; ++j) if (H[j] > best) best = H[j];
   return best;
 }
@@ -485,9 +497,11 @@ SB_HD bool rescue_mate_passes(const Params& p, int32_t score, uint32_t L) {
   return score > NEG_SCORE && (double)score >= p.min_score_fraction * (double)(p.ma * (int32_t)L);
 }
 // edit limit K: every edit costs at least min(ma - mp, ge) against a perfect score, so a place with more than K edits
-// cannot pass rescue_mate_passes
+// cannot pass rescue_mate_passes.  With clipping (softclip 1 or 2) a base left unaligned costs ma, which the search
+// counts as one edit, so ma joins the minimum.
 SB_HD int32_t rescue_edit_limit(const Params& p, uint32_t L) {
-  const int32_t per = (p.ma - p.mp) < p.ge ? (p.ma - p.mp) : p.ge;
+  int32_t per = (p.ma - p.mp) < p.ge ? (p.ma - p.mp) : p.ge;
+  if (p.softclip != 0 && p.ma < per) per = p.ma;
   if (per <= 0) return (int32_t)L;
   const double k = (1.0 - p.min_score_fraction) * (double)p.ma * (double)L / (double)per;
   if (!(k >= 0)) return 0;

@@ -637,6 +637,9 @@ __device__ __forceinline__ uint8_t base_code(uint8_t c, int ascii) {   // same m
   const uint8_t u = c & 0xDFu;
   return (u == 'A') ? 0 : (u == 'C') ? 1 : (u == 'G') ? 2 : (u == 'T') ? 3 : 4;
 }
+// MODE = Params::softclip (dp_score_serial): 1 lets a path start in the cell of column 0 and end in the cell of column
+// tlen-1 at any row, 2 lets any live cell start (diagonal predecessor floored at 0) and end a path.
+template <int MODE>
 __device__ __forceinline__ int32_t dp_warp_bytes(const IndexView& ix, const Params& p, const uint8_t* read, uint32_t L,
                                                  const Cand& c, uint32_t lane, int ascii) {
   const int32_t B = (int32_t)p.band, W = 2 * B + 1;
@@ -645,6 +648,7 @@ __device__ __forceinline__ int32_t dp_warp_bytes(const IndexView& ix, const Para
   const uint8_t* ref = ix.codes + ix.tx_off[c.tid];
   const bool in_band = (int32_t)lane < W;
   int32_t H = in_band ? 0 : NEG_SCORE, E = NEG_SCORE;
+  int32_t top = NEG_SCORE;     // modes 1 and 2: the lane's best end before the last row
   int64_t rpos = (int64_t)c.diag_c + ((int32_t)lane - B);
   uint8_t rbase = (rpos >= 0 && rpos < tlen) ? ref[rpos] : (uint8_t)255;
   for (uint32_t i = 0; i < L; ++i) {
@@ -655,7 +659,9 @@ __device__ __forceinline__ int32_t dp_warp_bytes(const IndexView& ix, const Para
     const int32_t Eup = __shfl_down_sync(0xffffffffu, E, 1);
     int32_t m = NEG_SCORE, e = NEG_SCORE;
     if (valid) {
-      m = H + ((rb < 4 && rb == rbase) ? p.ma : p.mp);
+      int32_t hd = H;
+      if (MODE == 2 || (MODE == 1 && rpos == 0)) hd = max(hd, 0);
+      m = hd + ((rb < 4 && rb == rbase) ? p.ma : p.mp);
       if ((int32_t)lane + 1 < W) e = max(Hup - p.go - p.ge, Eup - p.ge);
       if (e < NEG_SCORE) e = NEG_SCORE;
     }
@@ -672,6 +678,7 @@ __device__ __forceinline__ int32_t dp_warp_bytes(const IndexView& ix, const Para
     if (f < NEG_SCORE) f = NEG_SCORE;
     int32_t h = NEG_SCORE;
     if (valid) { h = max(hp, f); if (h < NEG_SCORE) h = NEG_SCORE; }
+    if (MODE != 0 && valid && (MODE == 2 || rpos == tlen - 1)) top = max(top, h);
     H = h;
     E = valid ? e : NEG_SCORE;
     const uint8_t nb = __shfl_down_sync(0xffffffffu, rbase, 1);
@@ -680,6 +687,7 @@ __device__ __forceinline__ int32_t dp_warp_bytes(const IndexView& ix, const Para
     else rbase = nb;
   }
   int32_t best = in_band ? H : NEG_SCORE;
+  if (MODE != 0) best = max(best, top);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
   return best;
@@ -739,7 +747,20 @@ __device__ __forceinline__ void load_window(const IndexView& ix, int64_t tbase, 
 // the other 2*band diagonals; when the best ungapped score is within (go+ge) of a perfect score no gapped path can
 // beat it.  Otherwise the alignment goes to the interior list (whole band inside the transcript -> k_dp_pair) or the
 // edge list; anything touching an N goes to the byte-code list.  List slots are reserved once per warp.
-template <int NWR>   // read words: 4 (read_len <= 128) or 8 (<= 256)
+//
+// Why the shortcut is exact, per scoring mode (MODE = Params::softclip):
+//   Every path with a gap scores at most ma*L - go - ge = bound: a deletion costs go + ge with at most L bases matched,
+//   an insertion costs go + ge and leaves a base unmatched, and clipped bases (modes 1, 2) add nothing.  So when the
+//   best ungapped path of the band reaches the bound, it is the DP's score.
+//   mode 0: the ungapped paths are the diagonals that lie inside the transcript; the others are dead.
+//   mode 1: a diagonal that leaves the transcript is a valid path as well (its overhang is clipped), so only interior
+//           alignments (whole band inside the transcript) may take the shortcut; those score as in mode 0, since no band
+//           cell reaches column 0 after row 0 or column tlen-1 before the last row.  Mode 1 only changes the DP kernels'
+//           edge and N paths.
+//   mode 2: only interior alignments, and only a perfect diagonal settles the alignment: ma*L is the most any path can
+//           score, while a full-length diagonal with a mismatch may be beaten by a clipped run of the same diagonal, so
+//           the DP scores those.
+template <int NWR, int MODE>   // read words: 4 (read_len <= 128) or 8 (<= 256)
 __global__ void __launch_bounds__(256, 3)
 k_dp_classify(IndexView ix, Params p, PackedReads pr, uint32_t L, int fast_ok, DpIo io) {
   const uint32_t lane = threadIdx.x & 31u;
@@ -764,8 +785,10 @@ k_dp_classify(IndexView ix, Params p, PackedReads pr, uint32_t L, int fast_ok, D
       else {
         const int64_t tbase = (int64_t)ix.tx_off[c.tid];
         const int64_t tlen = (int64_t)ix.tx_off[c.tid + 1] - tbase;
+        const bool interior = ((int64_t)c.diag_c - B >= 0) && ((int64_t)c.diag_c + (int64_t)L + B <= tlen);
+        const bool try_fast = fast_ok && (MODE == 0 || interior);
         int32_t best_u = NEG_SCORE;
-        if (fast_ok) {
+        if (try_fast) {
           uint64_t rw[NWR];
           load_oriented_read<NWR>(pr, mi, L, c.ori_cov >> 31, rw);
           uint64_t ww[NWR + 2];
@@ -790,10 +813,9 @@ k_dp_classify(IndexView ix, Params p, PackedReads pr, uint32_t L, int fast_ok, D
             if (best_u == perfect) break;
           }
         }
-        if (fast_ok && best_u >= bound) {
+        if (try_fast && best_u >= (MODE == 2 ? perfect : bound)) {
           (mate ? io.score_r : io.score_l)[(size_t)r * MAXCAND + ci] = best_u;
         } else {
-          const bool interior = ((int64_t)c.diag_c - B >= 0) && ((int64_t)c.diag_c + (int64_t)L + B <= tlen);
           dest = interior ? 0 : 1;
         }
       }
@@ -820,9 +842,12 @@ k_dp_classify(IndexView ix, Params p, PackedReads pr, uint32_t L, int fast_ok, D
 // dp_score_serial; read and reference window live in registers (2-bit), no memory access in the row loop.  Dead
 // cells carry values around NEG_SCORE without re-clamping: they stay below -2^27, which every consumer treats
 // like NEG_SCORE (the hit is invalid), and never reach a live cell's maximum.
-template <int NWR>
+// MODE 2 (soft-clip): diagonal predecessors floored at 0 and the best cell of any row.  Interior alignments score the
+// same in modes 0 and 1 (k_dp_classify), so mode 1 runs the MODE 0 instance.
+template <int NWR, int MODE>
 __global__ void __launch_bounds__(256, 3)
 k_dp_pair(IndexView ix, Params p, PackedReads pr, uint32_t L, DpIo io) {
+  static_assert(MODE == 0 || MODE == 2, "interior alignments: mode 1 scores as mode 0");
   const uint32_t lane = threadIdx.x & 31u, hl = lane & 15u, half = lane >> 4;
   const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
   const uint32_t n = io.list_n[0];
@@ -841,6 +866,7 @@ k_dp_pair(IndexView ix, Params p, PackedReads pr, uint32_t L, DpIo io) {
     uint64_t ww[NWR + 2];
     load_window<NWR>(ix, (int64_t)ix.tx_off[c.tid], c.diag_c, B, ww);
     int32_t H0 = 0, H1 = last ? NEG_SCORE : 0, E0 = NEG_SCORE, E1 = NEG_SCORE;
+    int32_t top = NEG_SCORE;   // mode 2: the lane's best cell of any row
     // blocks of 16 rows: the lane's reference bases for rows r0 .. r0+15 are window indices r0 + 2hl (+1) ...
 #pragma unroll
     for (int blk = 0; blk < 2 * NWR; ++blk) {
@@ -864,8 +890,8 @@ k_dp_pair(IndexView ix, Params p, PackedReads pr, uint32_t L, DpIo io) {
         const int32_t En = __shfl_down_sync(0xffffffffu, E0, 1, 16);
         const int32_t e0 = max(H1 - goe, E1 - ge);
         int32_t e1 = max(Hn - goe, En - ge);
-        int32_t hp0 = max(H0 + s0, e0);
-        int32_t hp1 = max(H1 + s1, e1);
+        int32_t hp0 = max((MODE == 2 ? max(H0, 0) : H0) + s0, e0);
+        int32_t hp1 = max((MODE == 2 ? max(H1, 0) : H1) + s1, e1);
         if (last) { e1 = NEG_SCORE; hp1 = NEG_SCORE; }
         const int32_t x0 = hp0 + kge0, x1 = hp1 + kge1;
         int32_t inc = max(x0, x1);
@@ -882,9 +908,11 @@ k_dp_pair(IndexView ix, Params p, PackedReads pr, uint32_t L, DpIo io) {
         H1 = last ? NEG_SCORE : max(hp1, f1);
         E0 = e0; E1 = e1;
         rb0 = rb1;
+        if (MODE == 2) top = max(top, max(H0, H1));
       }
     }
     int32_t best = max(H0, H1);
+    if (MODE == 2) best = max(best, top);
 #pragma unroll
     for (int o = 8; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o, 16));
     if (best < -(1 << 27)) best = NEG_SCORE;
@@ -893,8 +921,8 @@ k_dp_pair(IndexView ix, Params p, PackedReads pr, uint32_t L, DpIo io) {
 }
 
 // k_dp_general: the rare rest -- alignments whose band leaves the transcript (register form with per-cell validity)
-// and alignments touching an N (byte form).  One warp per alignment, lanes = band cells.
-template <int NWR>
+// and alignments touching an N (byte form).  One warp per alignment, lanes = band cells.  MODE as in dp_warp_bytes.
+template <int NWR, int MODE>
 __global__ void __launch_bounds__(256, 3)
 k_dp_general(IndexView ix, Params p, PackedReads pr, const uint8_t* __restrict__ left,
              const uint8_t* __restrict__ right, uint32_t L, int ascii, DpIo io) {
@@ -910,7 +938,7 @@ k_dp_general(IndexView ix, Params p, PackedReads pr, const uint8_t* __restrict__
     const Cand c = mate ? io.cand_r[(size_t)r * MAXCAND + ci] : io.cand_l[(size_t)r * MAXCAND + ci];
     int32_t* out = (mate ? io.score_r : io.score_l) + (size_t)r * MAXCAND + ci;
     if (bytes) {
-      const int32_t s = dp_warp_bytes(ix, p, (mate ? right : left) + (size_t)r * L, L, c, lane, ascii);
+      const int32_t s = dp_warp_bytes<MODE>(ix, p, (mate ? right : left) + (size_t)r * L, L, c, lane, ascii);
       if (lane == 0) *out = s;
       continue;
     }
@@ -923,6 +951,7 @@ k_dp_general(IndexView ix, Params p, PackedReads pr, const uint8_t* __restrict__
     load_window<NWR>(ix, tbase, c.diag_c, B, ww);
     const bool in_band = (int32_t)lane < W;
     int32_t H = in_band ? 0 : NEG_SCORE, E = NEG_SCORE;
+    int32_t top = NEG_SCORE;   // modes 1 and 2: the lane's best end before the last row
     int64_t rpos = (int64_t)c.diag_c + ((int32_t)lane - B);
     uint32_t rbase = (rpos >= 0 && rpos < tlen) ? (uint32_t)((ww[0] >> (2 * lane)) & 3ull) : 255u;
     // stream of the bases entering at the last band lane: window index W, W+1, ...
@@ -943,7 +972,9 @@ k_dp_general(IndexView ix, Params p, PackedReads pr, const uint8_t* __restrict__
         const int32_t Eup = __shfl_down_sync(0xffffffffu, E, 1);
         int32_t mval = NEG_SCORE, e = NEG_SCORE;
         if (valid) {
-          mval = H + ((rb == rbase) ? p.ma : p.mp);
+          int32_t hd = H;
+          if (MODE == 2 || (MODE == 1 && rpos == 0)) hd = max(hd, 0);
+          mval = hd + ((rb == rbase) ? p.ma : p.mp);
           if ((int32_t)lane + 1 < W) e = max(Hup - p.go - p.ge, Eup - p.ge);
           if (e < NEG_SCORE) e = NEG_SCORE;
         }
@@ -960,6 +991,7 @@ k_dp_general(IndexView ix, Params p, PackedReads pr, const uint8_t* __restrict__
         if (f < NEG_SCORE) f = NEG_SCORE;
         int32_t h = NEG_SCORE;
         if (valid) { h = max(hp, f); if (h < NEG_SCORE) h = NEG_SCORE; }
+        if (MODE != 0 && valid && (MODE == 2 || rpos == tlen - 1)) top = max(top, h);
         H = h;
         E = valid ? e : NEG_SCORE;
         const uint32_t nb = __shfl_down_sync(0xffffffffu, rbase, 1);
@@ -970,6 +1002,7 @@ k_dp_general(IndexView ix, Params p, PackedReads pr, const uint8_t* __restrict__
       }
     }
     int32_t best = in_band ? H : NEG_SCORE;
+    if (MODE != 0) best = max(best, top);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
     if (lane == 0) *out = best;

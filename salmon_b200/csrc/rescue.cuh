@@ -102,6 +102,7 @@ __global__ void k_rescue_search(IndexView ix, Params p, PackedReads pr, uint32_t
   }
 }
 
+template <int MODE>   // Params::softclip
 __global__ void k_rescue_score(IndexView ix, Params p, const uint8_t* __restrict__ left, const uint8_t* __restrict__ right,
                                uint32_t L, int ascii, const Cand* __restrict__ cand_l, const Cand* __restrict__ cand_r,
                                RescueBufs rb) {
@@ -113,7 +114,7 @@ __global__ void k_rescue_score(IndexView ix, Params p, const uint8_t* __restrict
     const uint32_t r = task >> 8, side = (task >> 7) & 1u, c = task & 127u;
     const Cand a = (side ? cand_r : cand_l)[(size_t)r * MAXCAND + c];
     const Cand res = rescue_cand(a, rb.diag[t]);
-    const int32_t s = dp_warp_bytes(ix, p, (side ? left : right) + (size_t)r * L, L, res, lane, ascii);
+    const int32_t s = dp_warp_bytes<MODE>(ix, p, (side ? left : right) + (size_t)r * L, L, res, lane, ascii);
     if (lane == 0) rb.score[t] = s;
   }
 }

@@ -142,7 +142,8 @@ def _quantify(index, ctx, ep, device, dist, names, out_dir, dump_eq, dump_eq_wei
 
 def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=None, device=0, batch=262_144,
                 max_read_len=256, threads=8, dist=None, dump_eq=False, dump_eq_weights=False, num_bootstraps=0, seed=0,
-                write_mappings=None, write_qualities=False, write_unmapped_names=False, cmdline="", recover_orphans=False):
+                write_mappings=None, write_qualities=False, write_unmapped_names=False, cmdline="", recover_orphans=False,
+                softclip=0):
     """`salmon quant -i index -l IU -1 mates1 -2 mates2 -o out_dir` for the hot path: FASTQ/FASTA(.gz) files ->
     sb_reads_bucketed -> sb_map_batch -> ... -> quant.sf.  index: an _capi.Index or the path of a saved one.  With
     torch.distributed initialised every rank takes the global batches g with g % world == rank (round-robin sharding
@@ -150,12 +151,16 @@ def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=
     A pair whose mates differ in length is mapped at the shorter length (documented deviation until the kernels take
     per-mate lengths).  write_mappings: path of a SAM file of the mappings (`--writeMappings=FILE`), with the reads'
     qualities when write_qualities; write_unmapped_names: out_dir/aux_info/unmapped_names.txt.  Both need one GPU.
-    recover_orphans: `--recoverOrphans` (sets map_params.recover_orphans; single-end reads: no effect)."""
+    recover_orphans: `--recoverOrphans` (sets map_params.recover_orphans; single-end reads: no effect).
+    softclip: scoring mode of the DP (sets map_params.softclip when non-zero): 1 = `--softclipOverhangs`, 2 =
+    `--softclip` (DESIGN.md section 12)."""
     if isinstance(index, (str, bytes, os.PathLike)):
         index = _capi.Index.load(index)
     mp = map_params or map_default_params()
     if recover_orphans:
         mp.recover_orphans = 1
+    if softclip:
+        mp.softclip = int(softclip)
     meta = index.meta()
     if meta["first_decoy"] < index.n_txps:
         mp.first_decoy = meta["first_decoy"]

@@ -133,7 +133,8 @@ typedef int (*sb_sample_cb)(const double* alpha, uint32_t n_txps, void* user);
  * Returns 1 where doBootstrap returns false (:521-525). */
 int sb_bootstrap(sb_em_ctx* ctx, const sb_em_params* p, double num_mapped_frags,
                  uint32_t n_bootstraps, uint64_t seed, sb_sample_cb cb, void* user);
-/* Parity tap: per input class, the count drawn by the last replicate. */
+/* Parity tap: per input class, the count drawn by the last replicate.  Single-transcript classes
+ * on the same transcript share one count: each of them reports what all of them drew together. */
 int sb_bootstrap_last_counts(sb_em_ctx* ctx, uint64_t* counts_out);
 
 /* Replaces CollapsedGibbsSampler::sample (CollapsedGibbsSampler.hpp:18-21;
@@ -144,6 +145,11 @@ int sb_bootstrap_last_counts(sb_em_ctx* ctx, uint64_t* counts_out);
 int sb_gibbs(sb_em_ctx* ctx, const double* alphas_init, int use_vbem, int per_txp_prior,
              double vb_prior, uint32_t n_samples, uint32_t thinning, int no_gamma_draw,
              double num_mapped_frags, uint64_t seed, sb_sample_cb cb, void* user);
+/* Parity tap: the per-transcript state the last Gibbs round left, M doubles each.  mu_out: the
+ * gamma draws (count+prior ~ Gamma, scale 1/(0.1+effLen)) or, with no_gamma_draw, the means
+ * (count+prior)/effLen; 0 for inactive transcripts.  cnt_out: the counts that round's singletons
+ * and category draws produced.  SB_ERR_STATE if no sb_gibbs has run on the current table. */
+int sb_gibbs_last_state(sb_em_ctx* ctx, double* mu_out, double* cnt_out);
 
 /* ---- output seam (host code): the reference's file formats ---------------------------------
  * TPM as GZipWriter::writeAbundances computes it (src/output/GZipWriter.cpp:719-736). */

@@ -613,6 +613,8 @@ static double gamma_mt(double shape, double scale, uint32_t i, uint32_t round,
   double a = shape, boost = 1.0;
   uint32_t attempt = 0;
   uint32_t r[4];
+  /* no gamma distribution, and the loop below would never accept (the device returns NaN too) */
+  if (!(shape > 0.0) || isinf(shape)) return NAN;
   if (a < 1.0) {
     orc_philox4x32(i, 0xFFFFFFFFu, round, 2u, k0, k1, r);
     double u = u53(r[1], r[0]);
@@ -636,6 +638,11 @@ static double gamma_mt(double shape, double scale, uint32_t i, uint32_t round,
   }
 }
 
+double orc_gamma_draw(double shape, double scale, uint32_t i, uint32_t round,
+                      uint32_t k0, uint32_t k1) {
+  return gamma_mt(shape, scale, i, round, k0, k1);
+}
+
 int orc_gibbs(uint64_t C, uint32_t M, const uint64_t* off, const uint32_t* tids,
               const double* weights, const uint64_t* counts,
               const uint8_t* valid, const double* eff_len,
@@ -643,6 +650,19 @@ int orc_gibbs(uint64_t C, uint32_t M, const uint64_t* off, const uint32_t* tids,
               double vb_prior, uint32_t n_samples, uint32_t thinning,
               int no_gamma_draw, double num_mapped_frags, uint64_t seed,
               double* samples_out) {
+  return orc_gibbs_ex(C, M, off, tids, weights, counts, valid, eff_len, alphas_init,
+                      use_vbem, per_txp_prior_in, vb_prior, n_samples, thinning,
+                      no_gamma_draw, num_mapped_frags, seed, 0, samples_out, NULL, NULL);
+}
+
+int orc_gibbs_ex(uint64_t C, uint32_t M, const uint64_t* off, const uint32_t* tids,
+                 const double* weights, const uint64_t* counts,
+                 const uint8_t* valid, const double* eff_len,
+                 const double* alphas_init, int use_vbem, int per_txp_prior_in,
+                 double vb_prior, uint32_t n_samples, uint32_t thinning,
+                 int no_gamma_draw, double num_mapped_frags, uint64_t seed,
+                 uint32_t round0, double* samples_out, double* last_mu,
+                 double* last_cnt) {
   const double beta = 0.1;
   uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
   /* :357-371, :296-315 */
@@ -678,7 +698,7 @@ int orc_gibbs(uint64_t C, uint32_t M, const uint64_t* off, const uint32_t* tids,
   if (n_samples >= 100) nchains = 4;
   if (n_samples >= 200) nchains = 8;
   uint32_t step = n_samples / nchains;
-  uint32_t round_global = 0;
+  uint32_t round_global = round0;
   for (uint32_t sampleID = 0; sampleID < n_samples; ++sampleID) {
     /* :457-461 chain restarts at i*step, i>=1 */
     if (nchains > 1 && sampleID > 0 && sampleID % step == 0 && sampleID / step < nchains)
@@ -747,6 +767,8 @@ int orc_gibbs(uint64_t C, uint32_t M, const uint64_t* off, const uint32_t* tids,
       out[t] = (a > 1e-8) ? a : 0.0;
     }
   }
+  if (last_mu) memcpy(last_mu, mu, (size_t)M * sizeof(double));
+  if (last_cnt) memcpy(last_cnt, alphasIn, (size_t)M * sizeof(double));
   free(priorAlphas); free(alphasIn); free(alphasInit); free(mu); free(active); free(prob);
   return 0;
 }

@@ -131,6 +131,26 @@ int orc_gibbs(uint64_t C, uint32_t M, const uint64_t* off, const uint32_t* tids,
               int no_gamma_draw, double num_mapped_frags, uint64_t seed,
               double* samples_out /* n_samples*M */);
 
+/* orc_gibbs with two additions.  round0: the global round of the first draw, so that a
+ * call with round0 = k*thinning draws samples k, k+1, ... of a longer run started at
+ * round 0 (a split run's share; its chains restart from alphas_init as in orc_gibbs).
+ * last_mu / last_cnt (M each, may be NULL): mu and the drawn counts as the last round
+ * left them.  orc_gibbs is orc_gibbs_ex with round0 = 0 and no state outputs. */
+int orc_gibbs_ex(uint64_t C, uint32_t M, const uint64_t* off, const uint32_t* tids,
+                 const double* weights, const uint64_t* counts,
+                 const uint8_t* valid, const double* eff_len,
+                 const double* alphas_init, int use_vbem, int per_txp_prior,
+                 double vb_prior, uint32_t n_samples, uint32_t thinning,
+                 int no_gamma_draw, double num_mapped_frags, uint64_t seed,
+                 uint32_t round0, double* samples_out /* n_samples*M */,
+                 double* last_mu, double* last_cnt);
+
+/* One gamma draw of the Gibbs sampler (Marsaglia-Tsang with the shape < 1 boost): the
+ * draw for transcript i in global round `round` under the key (k0, k1).  Exposed so the
+ * draws can be checked against the gamma distribution and against the device. */
+double orc_gamma_draw(double shape, double scale, uint32_t i, uint32_t round,
+                      uint32_t k0, uint32_t k1);
+
 #ifdef __cplusplus
 }
 #endif

@@ -206,6 +206,7 @@ SYMBOLS = {
     "sb_bootstrap_last_counts": (C.c_int, [_P, _P]),
     "sb_gibbs": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_double, C.c_uint32, C.c_uint32, C.c_int, C.c_double,
                            C.c_uint64, _P, _P]),
+    "sb_gibbs_last_state": (C.c_int, [_P, _P, _P]),
     "sb_nccl_unique_id": (C.c_int, [_P]),
     "sb_em_comm_init": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "sb_em_comm_destroy": (C.c_int, [_P]),
@@ -492,6 +493,13 @@ class EMContext:
                                  n_samples, thinning, int(no_gamma_draw), float(num_mapped_frags), seed,
                                  C.cast(cb, C.c_void_p), None), "sb_gibbs")
         return np.array(samples)
+
+    def gibbs_last_state(self):
+        """sb_gibbs_last_state -> (mu [M], cnt [M]) as the last Gibbs round left them."""
+        mu = np.zeros(self.M, dtype=np.float64)
+        cnt = np.zeros(self.M, dtype=np.float64)
+        _check(self.lib.sb_gibbs_last_state(self.h, mu.ctypes.data, cnt.ctypes.data), "sb_gibbs_last_state")
+        return mu, cnt
 
     def arm_timeline(self, iteration: int) -> int:
         return _check(self.lib.sb_em_debug_timeline(self.h, None, iteration), "sb_em_debug_timeline")

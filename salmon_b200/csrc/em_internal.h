@@ -139,6 +139,7 @@ struct sb_em_ctx {
   uint8_t* d_valid_boot = nullptr;
   uint8_t* d_active = nullptr;
   double *d_gibbs_cnt = nullptr, *d_gibbs_mu = nullptr, *d_gibbs_prior = nullptr, *d_gibbs_out = nullptr;
+  uint32_t gibbs_m = 0;           // transcripts of the last sb_gibbs run (0: none has run); read by sb_gibbs_last_state
 
   // debug timeline
   unsigned long long* d_dbg = nullptr;

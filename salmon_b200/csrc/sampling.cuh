@@ -128,8 +128,8 @@ __global__ void k_boot_counts_out(uint64_t C, const uint32_t* __restrict__ cls_m
   uint64_t v = 0;
   const uint32_t m = cls_map[c];
   if (valid_boot[c] && m != 0xffffffffu) {
-    // several single-transcript classes on the same transcript share one accumulator:
-    // report it on the first of them only (tests use distinct labels).
+    // several single-transcript classes on the same transcript share one accumulator, and each
+    // of them reports it: the value is what all of them drew together.
     v = (m & 0x80000000u) ? samp_single[m & 0x7fffffffu] : samp_multi[m];
   }
   out[c] = v;
@@ -138,6 +138,9 @@ __global__ void k_boot_counts_out(uint64_t C, const uint32_t* __restrict__ cls_m
 // ---- Gibbs ------------------------------------------------------------------------
 __device__ double gamma_mt(double shape, double scale, uint32_t i, uint32_t round, uint32_t k0,
                            uint32_t k1) {
+  // a shape that is not a positive finite number has no gamma distribution, and the rejection
+  // loop below would never accept: return NaN so the sample shows it instead of hanging the kernel
+  if (!(shape > 0.0) || isinf(shape)) return nan("");
   double a = shape, boost = 1.0;
   uint32_t r[4];
   if (a < 1.0) {
@@ -386,6 +389,7 @@ extern "C" int sb_gibbs(sb_em_ctx* c, const double* alphas_init, int use_vbem, i
   const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
   k_gibbs_init<<<nblk(M, 256), 256, 0, st>>>(M, c->d_active, c->d_efflens, d_init, perTxp, prior,
                                               c->d_gibbs_prior, c->d_gibbs_cnt, c->d_gibbs_mu);
+  c->gibbs_m = M;
   std::vector<double> out(M);
   uint32_t round = c->sample_offset * thinning;   // a rank's share of a split run draws from its own rounds
   for (uint32_t sid = 0; sid < n_samples; ++sid) {
@@ -408,5 +412,16 @@ extern "C" int sb_gibbs(sb_em_ctx* c, const double* alphas_init, int use_vbem, i
     SB_CUDA(cudaStreamSynchronize(st));
     if (cb(out.data(), M, user) != 0) break;
   }
+  return SB_OK;
+}
+
+extern "C" int sb_gibbs_last_state(sb_em_ctx* c, double* mu_out, double* cnt_out) {
+  if (!c || !mu_out || !cnt_out) { set_error("null argument"); return SB_ERR_INVALID; }
+  if (!c->gibbs_m || c->gibbs_m != c->M) { set_error("no Gibbs run on the current table"); return SB_ERR_STATE; }
+  SB_CUDA(cudaSetDevice(c->device));
+  const size_t bytes = (size_t)c->M * 8;
+  SB_CUDA(cudaMemcpyAsync(mu_out, c->d_gibbs_mu, bytes, cudaMemcpyDeviceToHost, c->stream));
+  SB_CUDA(cudaMemcpyAsync(cnt_out, c->d_gibbs_cnt, bytes, cudaMemcpyDeviceToHost, c->stream));
+  SB_CUDA(cudaStreamSynchronize(c->stream));
   return SB_OK;
 }

@@ -176,6 +176,38 @@ def gibbs(eq, valid, eff_len, alphas_init, use_vbem, per_txp_prior, vb_prior, n_
     return out
 
 
+def gibbs_ex(eq, valid, eff_len, alphas_init, use_vbem, per_txp_prior, vb_prior, n_samples, thinning, no_gamma_draw,
+             num_mapped_frags, seed, round0=0):
+    """orc_gibbs_ex -> (samples [n_samples, M], mu and counts as the last round left them)."""
+    lib = load()
+    M = eq.n_txps
+    out = np.zeros((n_samples, M))
+    last_mu = np.zeros(M)
+    last_cnt = np.zeros(M)
+    rc = lib.orc_gibbs_ex(C.c_uint64(eq.n_classes), C.c_uint32(M), _p(eq.off), _p(eq.tids), _p(eq.weights),
+                          _p(eq.counts), _p(np.ascontiguousarray(valid, dtype=np.uint8)),
+                          _p(np.ascontiguousarray(eff_len, dtype=np.float64)),
+                          _p(np.ascontiguousarray(alphas_init, dtype=np.float64)), C.c_int(use_vbem),
+                          C.c_int(per_txp_prior), C.c_double(vb_prior), C.c_uint32(n_samples), C.c_uint32(thinning),
+                          C.c_int(no_gamma_draw), C.c_double(num_mapped_frags), C.c_uint64(seed), C.c_uint32(round0),
+                          _p(out), _p(last_mu), _p(last_cnt))
+    assert rc == 0
+    return out, last_mu, last_cnt
+
+
+def gamma_draws(shape, scale, idx, rnd, seed):
+    """orc_gamma_draw for every (shape, scale, i) triple: the sampler's gamma draws of round rnd."""
+    lib = load()
+    f = lib.orc_gamma_draw
+    f.restype = C.c_double
+    f.argtypes = [C.c_double, C.c_double, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
+    k0, k1 = seed & 0xFFFFFFFF, seed >> 32
+    shape, scale, idx = np.broadcast_arrays(np.asarray(shape, dtype=np.float64), np.asarray(scale, dtype=np.float64),
+                                            np.asarray(idx, dtype=np.uint64))
+    return np.array([f(float(a), float(s), int(i), rnd, k0, k1) for a, s, i in zip(shape.ravel(), scale.ravel(),
+                                                                                 idx.ravel())]).reshape(shape.shape)
+
+
 # ---------------------------------------------------------------------------- Stage A
 class orc_map_params(C.Structure):
     _fields_ = [

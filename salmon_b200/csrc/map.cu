@@ -684,7 +684,7 @@ __global__ void k_online_correction(uint32_t nf, OnlineState S, int cache, doubl
   S.cf[0] = 0.0;
   for (uint32_t i = 1; i < nf; ++i) {
     const double v = scratch[i];
-    vals = v * (double)i + vals;
+    vals = __dmul_rn(v, (double)i) + vals;       // no FMA: the product rounds as the reference's does
     mult = v + mult;
     S.cf[i] = (mult > 0) ? vals / mult : 0.0;
   }
@@ -1061,6 +1061,10 @@ static int dmalloc(T** p, size_t n) {
 }
 static inline unsigned nblk(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
 
+// the ungapped shortcut of k_dp_classify is exact only when no cell scores above ma and gaps cost something; under
+// other scores set_option("fast_dp", 1) leaves it off
+static inline int fast_dp_exact(const Params& p) { return (p.ma >= 0 && p.mp <= p.ma && p.go >= 0 && p.ge >= 0) ? 1 : 0; }
+
 // the three DP kernels of one chunk for scoring mode MODE (Params::softclip); the same launches in every mode
 template <int NWR, int MODE>
 static void launch_dp(const sb_map_ctx* c, cudaStream_t st, const IndexView& ix, const Params& p, uint32_t L,
@@ -1195,8 +1199,7 @@ extern "C" sb_map_ctx* sb_map_create(sb_index* ix, const sb_map_params* q, int d
     delete c;
     return nullptr;
   }
-  // the ungapped shortcut of k_dp_score_w needs: no cell scores above ma, gaps cost something
-  c->fast_ok = (p.ma >= 0 && p.mp <= p.ma && p.go >= 0 && p.ge >= 0) ? 1 : 0;
+  c->fast_ok = fast_dp_exact(p);
   cudaSetDevice(device);
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device);
@@ -1344,7 +1347,7 @@ extern "C" int sb_map_set_option(sb_map_ctx* c, const char* key, int64_t value) 
     c->variant = (int)value;
     return SB_OK;
   }
-  if (!strcmp(key, "fast_dp")) { c->fast_ok = value ? 1 : 0; return SB_OK; }
+  if (!strcmp(key, "fast_dp")) { c->fast_ok = (value && fast_dp_exact(c->p)) ? 1 : 0; return SB_OK; }
   if (!strcmp(key, "input_on_device")) { c->input_dev = value ? 1 : 0; return SB_OK; }
   if (!strcmp(key, "ascii_reads")) {
     if (value && c->variant == 0) { sb::set_error("ascii_reads needs the warp kernels (variant 1)"); return SB_ERR_INVALID; }

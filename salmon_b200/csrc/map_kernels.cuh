@@ -838,10 +838,12 @@ k_dp_classify(IndexView ix, Params p, PackedReads pr, uint32_t L, int fast_ok, D
 }
 
 // k_dp_pair: banded affine DP for interior alignments, TWO alignments per warp: a half-warp owns one alignment,
-// lane hl owns band cells 2*hl and 2*hl+1 (cell 31 does not exist and is kept dead).  Same recurrences as
-// dp_score_serial; read and reference window live in registers (2-bit), no memory access in the row loop.  Dead
-// cells carry values around NEG_SCORE without re-clamping: they stay below -2^27, which every consumer treats
-// like NEG_SCORE (the hit is invalid), and never reach a live cell's maximum.
+// lane hl owns band cells 2*hl and 2*hl+1.  The band has W = 2*band+1 cells; cells W..31 do not exist and are forced
+// dead in every row (cell 2*band+1 in lane band, both cells in the lanes above; at band 15 only cell 31): starting them
+// dead is not enough, F would carry live values rightward into them.  Same recurrences as dp_score_serial; read and
+// reference window live in registers (2-bit), no memory access in the row loop.  Values derived from dead cells (E, F
+// and the prefix scan) stay below -2^27 without re-clamping, which every consumer treats like NEG_SCORE (the hit is
+// invalid), and never reach a live cell's maximum.
 // MODE 2 (soft-clip): diagonal predecessors floored at 0 and the best cell of any row.  Interior alignments score the
 // same in modes 0 and 1 (k_dp_classify), so mode 1 runs the MODE 0 instance.
 template <int NWR, int MODE>
@@ -854,7 +856,7 @@ k_dp_pair(IndexView ix, Params p, PackedReads pr, uint32_t L, DpIo io) {
   const int32_t B = (int32_t)p.band;
   const int32_t goe = p.go + p.ge, ge = p.ge;
   const int32_t kge0 = (int32_t)(2 * hl) * ge, kge1 = kge0 + ge;
-  const bool last = hl == 15u;          // cell 30 | cell 31 (dead)
+  const bool dead0 = (int32_t)hl > B, dead1 = (int32_t)hl >= B;   // cells 2hl, 2hl+1 lie outside the band (>= W)
   for (uint32_t t2 = warp * 2; t2 < n; t2 += nwarps * 2) {
     const uint32_t t = (t2 + half < n) ? t2 + half : t2;       // odd tail: both halves do the same alignment
     const uint32_t task = io.list_int[t];
@@ -865,7 +867,7 @@ k_dp_pair(IndexView ix, Params p, PackedReads pr, uint32_t L, DpIo io) {
     load_oriented_read<NWR>(pr, mi, L, c.ori_cov >> 31, rw);
     uint64_t ww[NWR + 2];
     load_window<NWR>(ix, (int64_t)ix.tx_off[c.tid], c.diag_c, B, ww);
-    int32_t H0 = 0, H1 = last ? NEG_SCORE : 0, E0 = NEG_SCORE, E1 = NEG_SCORE;
+    int32_t H0 = dead0 ? NEG_SCORE : 0, H1 = dead1 ? NEG_SCORE : 0, E0 = NEG_SCORE, E1 = NEG_SCORE;
     int32_t top = NEG_SCORE;   // mode 2: the lane's best cell of any row
     // blocks of 16 rows: the lane's reference bases for rows r0 .. r0+15 are window indices r0 + 2hl (+1) ...
 #pragma unroll
@@ -892,7 +894,7 @@ k_dp_pair(IndexView ix, Params p, PackedReads pr, uint32_t L, DpIo io) {
         int32_t e1 = max(Hn - goe, En - ge);
         int32_t hp0 = max((MODE == 2 ? max(H0, 0) : H0) + s0, e0);
         int32_t hp1 = max((MODE == 2 ? max(H1, 0) : H1) + s1, e1);
-        if (last) { e1 = NEG_SCORE; hp1 = NEG_SCORE; }
+        if (dead1) { e1 = NEG_SCORE; hp1 = NEG_SCORE; }
         const int32_t x0 = hp0 + kge0, x1 = hp1 + kge1;
         int32_t inc = max(x0, x1);
 #pragma unroll
@@ -904,9 +906,9 @@ k_dp_pair(IndexView ix, Params p, PackedReads pr, uint32_t L, DpIo io) {
         if (hl == 0) exc = NEG_SCORE;
         const int32_t f0 = exc - p.go - kge0;
         const int32_t f1 = max(exc, x0) - p.go - kge1;
-        H0 = max(hp0, f0);
-        H1 = last ? NEG_SCORE : max(hp1, f1);
-        E0 = e0; E1 = e1;
+        H0 = dead0 ? NEG_SCORE : max(hp0, f0);
+        H1 = dead1 ? NEG_SCORE : max(hp1, f1);
+        E0 = dead0 ? NEG_SCORE : e0; E1 = e1;
         rb0 = rb1;
         if (MODE == 2) top = max(top, max(H0, H1));
       }

@@ -7,7 +7,8 @@ from salmon_b200._capi import Index, map_default_params
 from salmon_b200.synth import synth_reads, synth_txome
 
 
-def compare(a, b, cap):
+def compare(a, b, cap, binned=True):
+    """binned=False (range_bins 0): a label is its n_aln transcripts, the bin slots after them are not written"""
     assert np.array_equal(a["n_aln"], b["n_aln"])
     n = a["n_aln"].shape[0]
     m = np.arange(cap)[None, :] < a["n_aln"][:, None]
@@ -15,7 +16,7 @@ def compare(a, b, cap):
         assert np.array_equal(a[k][m], b[k][m]), k
     assert np.array_equal(a["prob"][m].view(np.uint64), b["prob"][m].view(np.uint64))
     assert np.array_equal(a["weight"][m].view(np.uint64), b["weight"][m].view(np.uint64))
-    m2 = np.arange(2 * cap)[None, :] < 2 * a["n_aln"][:, None]
+    m2 = np.arange(2 * cap)[None, :] < (2 if binned else 1) * a["n_aln"][:, None]
     assert np.array_equal(a["label"][m2], b["label"][m2])
 
 
@@ -123,15 +124,76 @@ def test_decoys_host_logic_matches_oracle(oracle):
     assert got2["counters"]["mapped"] > got["counters"]["mapped"]
 
 
-@pytest.mark.parametrize("master_seed", [1, 4])
-def test_fuzz_host_logic_against_oracle(oracle, master_seed):
-    """Randomised parity: adversarial transcriptomes (shared blocks, homopolymers, N, short references), read lengths
-    35..125, error rates up to 5 % / 2 % indels, and random settings of stride, maxReadOcc, maxOccsPerHit, range bins,
-    hard filter, minScoreFraction, consensus fraction, k, band, first decoy, fragLenDistMax, in all three regimes of the
-    fragment counter -- the product's per-read logic stays bit-exact with the oracle."""
+# indel lengths planted in mates: each band of the sweeps (0, 1, 2, 3, 7, 8, 14, 15) has a gap just inside and one just
+# outside its reach, and the longest ones lie beyond every band
+INDEL_LENS = (1, 2, 3, 5, 8, 9, 12, 15, 16, 20, 24)
+BANDS = (0, 1, 2, 3, 7, 8, 14, 15)
+# (ma, mp, go, ge): the default, and sets where m * (ma - mp) = go + ge has an integer solution m (1, 2, 1 mismatches
+# for the 2nd to 4th), i.e. an ungapped alignment with m mismatches lands exactly on the ungapped shortcut's bound
+SCORES = ((2, -4, 6, 2), (1, -1, 1, 1), (2, -2, 6, 2), (3, -3, 4, 2), (2, -4, 0, 1))
+_COMP5 = np.array([3, 2, 1, 0, 4], dtype=np.uint8)
+
+
+def tie_mismatches(ma, mp, go, ge):
+    """m with m * (ma - mp) == go + ge, or None"""
+    return (go + ge) // (ma - mp) if (go + ge) % (ma - mp) == 0 else None
+
+
+def plant_mate(src, L, rng, d=0, m=0):
+    """an L-base mate read from src (its source on the mate's own strand, continuing at least d bases past the mate's
+    end): with d > 0 one deletion or insertion of d bases at a random position or within 5 bases of either end; with
+    m > 0 exactly m substitutions at distinct positions; else the plain bases"""
+    src = np.asarray(src, dtype=np.uint8)
+    if d:
+        w = int(rng.integers(3))
+        p = int(rng.integers(1, L)) if w == 0 else (int(rng.integers(1, 6)) if w == 1 else L - int(rng.integers(1, 6)))
+        if rng.random() < 0.5:       # deletion: the mate skips d reference bases
+            out = np.concatenate([src[:p], src[p + d:L + d]])
+        else:                        # insertion of d random bases
+            out = np.concatenate([src[:p], rng.integers(0, 4, d, dtype=np.uint8), src[p:max(p, L - d)]])[:L]
+    else:
+        out = src[:L].copy()
+    if m:
+        q = rng.choice(L, m, replace=False)
+        out[q] = (out[q] + rng.integers(1, 4, m, dtype=np.uint8)) % 4
+    assert out.shape[0] == L
+    return out.astype(np.uint8)
+
+
+def planted_pairs(txps, rng, n, L, frag_mean, frag_sd=20.0, indel_frac=0.4, subs=(), sub_frac=0.0):
+    """n IU pairs from the transcripts of at least L + 48 bases; each mate independently carries one indel (length from
+    INDEL_LENS) with probability indel_frac, else exactly m substitutions (m from subs) with probability sub_frac"""
+    D = max(INDEL_LENS)
+    ok = np.flatnonzero(np.array([len(t) for t in txps]) >= L + 2 * D)
+    if len(ok) == 0:
+        raise ValueError("no transcript long enough")
+    left = np.zeros((n, L), np.uint8)
+    right = np.zeros((n, L), np.uint8)
+    for i in range(n):
+        t = txps[int(rng.choice(ok))]
+        tl = len(t)
+        fl = int(np.clip(round(rng.normal(frag_mean, frag_sd)), L, tl - 2 * D))
+        pos = int(rng.integers(D, tl - D - fl + 1))
+        mates = []
+        for src in (t[pos:pos + L + D], _COMP5[t[pos + fl - L - D:pos + fl][::-1]]):
+            u = rng.random()
+            d = int(rng.choice(INDEL_LENS)) if u < indel_frac else 0
+            m = int(rng.choice(subs)) if (subs and indel_frac <= u < indel_frac + sub_frac) else 0
+            mates.append(plant_mate(src, L, rng, d, m))
+        if rng.random() < 0.5:
+            mates.reverse()
+        left[i], right[i] = mates
+    return left, right
+
+
+def fuzz_trials(master_seed, n_trials, read_lens=(35, 50, 75, 100, 125, 150, 200, 256)):
+    """Randomised mapping trials: adversarial transcriptomes (shared blocks, homopolymers, N, short references), error
+    rates up to 5 % / 2 % one-base indels, planted indels of up to 24 bases, and random settings of stride, maxReadOcc,
+    maxOccsPerHit, range bins, hard filter, minScoreFraction, consensus fraction, k, band, scores, first decoy,
+    fragLenDistMax and the fragment counter.  Yields dict(txps, left, right, L, over, frag_counter); the stride keeps
+    (L - k) / stride + 2 within the 64 seed positions a GPU context takes."""
     rng = np.random.default_rng(master_seed)
-    done = 0
-    for trial in range(70):
+    for trial in range(n_trials):
         seed = int(rng.integers(1, 1 << 30))
         if trial % 4 == 0:
             txps, _ = synth_txome(seed=seed, n_genes=int(rng.integers(5, 40)))
@@ -153,16 +215,23 @@ def test_fuzz_host_logic_against_oracle(oracle, master_seed):
                 if r.random() < 0.2:
                     t[int(r.integers(0, len(t)))] = 4
                 txps.append(t)
-            if max(len(t) for t in txps) < 150:
-                txps.append(r.integers(0, 4, size=400, dtype=np.uint8))
-        L = int(rng.choice([35, 50, 75, 100, 125]))
-        fm = float(rng.choice([max(L + 20, 120), 250]))
+        L = int(rng.choice(read_lens))
+        if max(len(t) for t in txps) < max(150, L + 60):
+            txps.append(np.random.default_rng(seed + 2).integers(0, 4, size=max(400, 2 * L + 60), dtype=np.uint8))
+        fm = float(rng.choice([max(L + 20, 120), max(250, L + 40)]))
         try:
             left, right, _ = synth_reads(txps, seed=seed + 1, n=int(rng.integers(50, 300)), read_len=L, frag_mean=fm,
                                          frag_sd=float(rng.choice([5, 25])), sub_rate=float(rng.choice([0.0, 0.01, 0.05])),
                                          indel_rate=float(rng.choice([0.0, 0.003, 0.02])), random_frac=0.1)
         except Exception:  # noqa: BLE001  (the simulator refuses transcriptomes shorter than its fragments)
             continue
+        if rng.random() < 0.5:    # a third of the pairs replaced by pairs with planted multi-base indels
+            sel = rng.choice(left.shape[0], left.shape[0] // 3, replace=False)
+            try:
+                left[sel], right[sel] = planted_pairs(txps, np.random.default_rng(seed + 3), len(sel), L, fm,
+                                                      indel_frac=0.7)
+            except ValueError:
+                pass
         if rng.random() < 0.3:
             left[rng.integers(0, left.shape[0]), rng.integers(0, L)] = 4
         over = {}
@@ -170,13 +239,30 @@ def test_fuzz_host_logic_against_oracle(oracle, master_seed):
                                     ("max_occs_per_hit", 0.4, [1, 3, 16, 200]), ("range_bins", 0.4, [0, 1, 8]),
                                     ("hard_filter", 0.3, [1]), ("min_score_fraction", 0.3, [0.3, 0.8, 0.95]),
                                     ("consensus_frac", 0.3, [0.3, 0.9, 1.0]), ("k", 0.3, [15, 21, 25]),
-                                    ("band", 0.3, [3, 8, 15]), ("max_frag_len", 0.3, [200, 400])):
+                                    ("band", 0.4, list(BANDS)), ("max_frag_len", 0.3, [200, 400])):
             if rng.random() < p_use:
                 v = rng.choice(choices)
                 over[key] = float(v) if isinstance(choices[0], float) else int(v)
+        if rng.random() < 0.3:
+            over.update(zip(("ma", "mp", "go", "ge"), SCORES[int(rng.integers(len(SCORES)))]))
         if rng.random() < 0.2:
             over["first_decoy"] = max(1, len(txps) - int(rng.integers(1, 4)))
-        run_both(oracle, txps, left, right, frag_counter=int(rng.choice([0, 0, 6000, 6_000_000])), **over)
+        k, stride = over.get("k", 31), over.get("stride", 4)
+        while (L - k) // stride + 2 > 64:
+            stride += 1
+        if stride != over.get("stride", 4):
+            over["stride"] = stride
+        yield dict(txps=txps, left=left, right=right, L=L, over=over,
+                   frag_counter=int(rng.choice([0, 0, 6000, 6_000_000])))
+
+
+@pytest.mark.parametrize("master_seed", [1, 4])
+def test_fuzz_host_logic_against_oracle(oracle, master_seed):
+    """Randomised parity (fuzz_trials): the product's per-read logic stays bit-exact with the oracle, in all three
+    regimes of the fragment counter."""
+    done = 0
+    for t in fuzz_trials(master_seed, 70):
+        run_both(oracle, t["txps"], t["left"], t["right"], frag_counter=t["frag_counter"], **t["over"])
         done += 1
     assert done >= 40
 

@@ -310,6 +310,18 @@ typedef struct sb_map_params {
    * band; includes 1).  The acceptance threshold stays minScoreFraction * ma * read length.  Other values are refused;
    * variant 0 of the mapping kernels supports 0 only. */
   int32_t softclip;
+  /* fragment likelihood of each kept mapping (rule: DESIGN.md section 13); all zero = salmon's defaults.
+   * no_single_frag_prob (--noSingleFragProb): an orphan of a paired-end library gets log P = LOG_EPSILON and a single-end
+   * read LOG_1 instead of the ambiguous-length probability.  no_frag_len_dist (--noFragLengthDist): no fragment-length
+   * term at all (orphans and single-end reads as under no_single_frag_prob); needs no_eff_len_correction.
+   * no_eff_len_correction (--noEffectiveLengthCorrection): transcript lengths replace effective lengths in the online
+   * phase after burn-in and in sb_map_result.eff_len (what the optimiser, the samplers and quant.sf take). */
+  int32_t no_single_frag_prob;
+  int32_t no_frag_len_dist;
+  int32_t no_eff_len_correction;
+  /* --incompatPrior as a probability: 0 (or below 1e-100) = mappings incompatible with lib_type are ignored (the
+   * default); otherwise they stay in and carry log(incompat_prior) in their auxiliary probability.  In [0, 1]. */
+  double incompat_prior;
 } sb_map_params;
 /* Only sb_quant_files takes these two: the library type is detected from the first 50 000 fragments that show a
  * strand, as LibraryTypeDetector does (include/salmon/internal/model/LibraryTypeDetector.hpp:34-140): until then every
@@ -338,6 +350,7 @@ typedef struct sb_map_batch_stats {
   uint64_t orphans_rescued, rescue_searches, rescue_no_room;
   float rescue_kernel_ms;
   uint32_t reserved2;
+  uint64_t compatible;        /* mapped fragments with at least one kept mapping compatible with lib_type */
 } sb_map_batch_stats;
 
 typedef struct sb_map_result {   /* host CSR owned by the context, valid until destroy / next finish */
@@ -360,6 +373,7 @@ typedef struct sb_map_result {   /* host CSR owned by the context, valid until d
    * mapped forward), [3] SR; [4..7] reserved */
   uint64_t lib_format_counts[8];
   uint64_t orphans_rescued, rescue_searches, rescue_no_room;   /* sums of sb_map_batch_stats' fields since create / reset */
+  uint64_t n_compatible;           /* sum of sb_map_batch_stats.compatible (sb_map_reduce_global: over all ranks) */
 } sb_map_result;
 
 typedef struct sb_map_ctx sb_map_ctx;
@@ -392,6 +406,7 @@ typedef struct sb_map_partial {
   const uint64_t* cluster_hits;    /* [n_txps] fragments whose first transcript this is */
   const uint32_t* cluster_root;    /* [n_txps] smallest transcript id of the transcript's cluster */
   uint64_t assigned;               /* fragments assigned by this rank */
+  uint64_t compatible;             /* of those, fragments with a kept mapping compatible with the library type */
 } sb_map_partial;
 int sb_map_partial_get(sb_map_ctx* ctx, sb_map_partial* out);
 int sb_map_project_global(sb_map_ctx* ctx, const sb_map_partial* global_stats, uint32_t n_ranks,

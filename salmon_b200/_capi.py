@@ -84,6 +84,8 @@ class sb_map_params(C.Structure):
         ("pre_merge_thresh", C.c_double), ("post_merge_thresh", C.c_double), ("orphan_thresh", C.c_double),
         ("allow_dovetail", C.c_int32), ("allow_orphans", C.c_int32), ("lib_type", C.c_int32),
         ("recover_orphans", C.c_int32), ("softclip", C.c_int32),
+        ("no_single_frag_prob", C.c_int32), ("no_frag_len_dist", C.c_int32), ("no_eff_len_correction", C.c_int32),
+        ("incompat_prior", C.c_double),
     ]
 
 
@@ -93,7 +95,7 @@ class sb_map_batch_stats(C.Structure):
                                    "n_batch_classes")] + [("device_ms", C.c_float), ("reserved", C.c_uint32), ("full_dp", C.c_uint64),
                                                               ("seed_kernel_ms", C.c_float), ("seed_kernel_launches", C.c_uint32)] + \
         [(k, C.c_uint64) for k in ("orphans_rescued", "rescue_searches", "rescue_no_room")] + \
-        [("rescue_kernel_ms", C.c_float), ("reserved2", C.c_uint32)]
+        [("rescue_kernel_ms", C.c_float), ("reserved2", C.c_uint32), ("compatible", C.c_uint64)]
 
     def asdict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
@@ -106,7 +108,7 @@ class sb_map_result(C.Structure):
         [("n_txps", C.c_uint32), ("reserved", C.c_uint32), ("projected_counts", C.POINTER(C.c_double)),
          ("eff_len", C.POINTER(C.c_double)), ("unique_counts", C.POINTER(C.c_uint64)),
          ("total_counts", C.POINTER(C.c_uint64)), ("lib_format_counts", C.c_uint64 * 8)] + \
-        [(k, C.c_uint64) for k in ("orphans_rescued", "rescue_searches", "rescue_no_room")]
+        [(k, C.c_uint64) for k in ("orphans_rescued", "rescue_searches", "rescue_no_room", "n_compatible")]
 
 
 # every symbol include/salmon_b200.h declares: (name, restype, argtypes)
@@ -116,7 +118,8 @@ class sb_map_partial(C.Structure):
                 ("fld_hist", C.POINTER(C.c_double)), ("fld_tot", C.c_double), ("fld_prior_hist", C.POINTER(C.c_double)),
                 ("fld_prior_tot", C.c_double), ("fld_min", C.c_uint32), ("reserved", C.c_uint32),
                 ("unique_counts", C.POINTER(C.c_uint64)), ("total_counts", C.POINTER(C.c_uint64)),
-                ("cluster_hits", C.POINTER(C.c_uint64)), ("cluster_root", C.POINTER(C.c_uint32)), ("assigned", C.c_uint64)]
+                ("cluster_hits", C.POINTER(C.c_uint64)), ("cluster_root", C.POINTER(C.c_uint32)), ("assigned", C.c_uint64),
+                ("compatible", C.c_uint64)]
 
 
 class sb_eq_file(C.Structure):
@@ -726,7 +729,8 @@ class MapContext:
                     fld_prior_hist=arr(q.fld_prior_hist, nf, np.float64), fld_prior_tot=float(q.fld_prior_tot),
                     fld_min=int(q.fld_min), unique_counts=arr(q.unique_counts, M, np.uint64),
                     total_counts=arr(q.total_counts, M, np.uint64), cluster_hits=arr(q.cluster_hits, M, np.uint64),
-                    cluster_root=arr(q.cluster_root, M, np.uint32), assigned=int(q.assigned))
+                    cluster_root=arr(q.cluster_root, M, np.uint32), assigned=int(q.assigned),
+                    compatible=int(q.compatible))
 
     def project_global(self, g: dict, roots_all: np.ndarray) -> dict:
         """normalizeAlphas with the statistics reduced over all ranks; returns the per-transcript EM inputs"""
@@ -743,7 +747,7 @@ class MapContext:
         q.unique_counts = keep["unique_counts"].ctypes.data_as(C.POINTER(C.c_uint64))
         q.total_counts = keep["total_counts"].ctypes.data_as(C.POINTER(C.c_uint64))
         q.cluster_hits = keep["cluster_hits"].ctypes.data_as(C.POINTER(C.c_uint64))
-        q.cluster_root = None; q.assigned = int(g["assigned"])
+        q.cluster_root = None; q.assigned = int(g["assigned"]); q.compatible = int(g.get("compatible", 0))
         r = sb_map_result()
         _check(self.lib.sb_map_project_global(self.h, C.byref(q), roots_all.shape[0], roots_all.ctypes.data, C.byref(r)),
                "sb_map_project_global")
@@ -781,6 +785,7 @@ class MapContext:
             out[k] = np.ctypeslib.as_array(getattr(r, k), shape=(M,)).copy() if M else np.zeros(0, dt)
         out["lib_format_counts"] = dict(zip(("ISF", "ISR", "SF", "SR"), [int(x) for x in r.lib_format_counts[:4]]))
         out["rescue"] = {k: int(getattr(r, k)) for k in ("orphans_rescued", "rescue_searches", "rescue_no_room")}
+        out["counters"]["n_compatible"] = int(r.n_compatible)
         return out
 
     def online_state(self):

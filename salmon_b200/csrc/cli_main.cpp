@@ -75,7 +75,8 @@ int usage() {
           "  sb_salmon index -t transcripts.fa[.gz] -i index_dir [-k 31] [--gencode] [-d decoys.txt] [--keepDuplicates] [--no-clip]\n"
           "  sb_salmon quant -i index_dir -l IU|ISF|ISR -1 r1.fq[.gz] ... -2 r2.fq[.gz] ... | -l U|SF|SR -r reads.fq[.gz] ...  -o out_dir [--gpus N]\n"
           "                  [-p threads] [--dumpEq] [--dumpEqWeights] [--writeMappings[=FILE] | -z] [--writeQualities] [--writeUnmappedNames]\n"
-          "                  [--recoverOrphans] [--softclip] [--softclipOverhangs]\n"
+          "                  [--recoverOrphans] [--softclip] [--softclipOverhangs] [--incompatPrior 0] [--noSingleFragProb]\n"
+          "                  [--noFragLengthDist --noEffectiveLengthCorrection | --noEffectiveLengthCorrection]\n"
           "                  [--numBootstraps N | --numGibbsSamples N] [--thinningFactor 16] [--noGammaDraw] [--useEM] [--vbPrior 0.01]\n"
           "                  [--perNucleotidePrior] [--maxReadOcc 200] [--maxOccsPerHit 1000] [--minScoreFraction 0.65] [--consensusSlack 0.35]\n"
           "                  [--preMergeChainSubThresh 0.75] [--postMergeChainSubThresh 0.9] [--orphanChainSubThresh 0.95] [--allowDovetail]\n"
@@ -277,6 +278,20 @@ int cmd_quant(Args& a) {
     else if (o == "--writeQualities") qo.write_qualities = 1;
     else if (o == "--writeUnmappedNames") qo.write_unmapped_names = 1;
     else if (o == "--recoverOrphans") mp.recover_orphans = 1;
+    else if (o == "--incompatPrior") {
+      if (!a.value(v)) return usage();
+      char* end = nullptr;
+      const double x = strtod(v.c_str(), &end);
+      if (v.empty() || *end != '\0' || !(x >= 0.0 && x <= 1.0)) {
+        fprintf(stderr, "sb_salmon quant: --incompatPrior takes a probability in [0, 1], got '%s'\n", v.c_str());
+        return 1;
+      }
+      // 0 or below 1e-100: incompatible mappings are ignored (QuantOptionsUtils.cpp:608-616)
+      mp.incompat_prior = (x == 0.0 || x < 1e-100) ? 0.0 : x;
+    }
+    else if (o == "--noSingleFragProb") mp.no_single_frag_prob = 1;
+    else if (o == "--noFragLengthDist") mp.no_frag_len_dist = 1;
+    else if (o == "--noEffectiveLengthCorrection") mp.no_eff_len_correction = 1;
     else if (o == "--seqBias" || o == "--gcBias" || o == "--posBias" || o == "-a" ||
              o == "--alignments" || o == "-g" || o == "--geneMap" || o == "--sketchMode") {
       fprintf(stderr, "sb_salmon quant: %s is outside the hot path this build replaces (DESIGN.md, out of scope)\n", o.c_str());
@@ -284,6 +299,10 @@ int cmd_quant(Args& a) {
     } else { fprintf(stderr, "sb_salmon quant: unknown option %s\n", o.c_str()); return usage(); }
   }
   if (out.empty()) return usage();
+  if (mp.no_frag_len_dist && !mp.no_eff_len_correction) {   // QuantOptionsUtils.cpp:641-647
+    fprintf(stderr, "sb_salmon quant: You cannot enable --noFragLengthDist without also enabling --noEffectiveLengthCorrection\n");
+    return 1;
+  }
   if (n_gpus > 1 && (!sam_path.empty() || qo.write_unmapped_names)) {
     fprintf(stderr, "sb_salmon quant: --writeMappings / --writeUnmappedNames are written by a one-GPU run only: a read-sharded "
                     "--gpus %d run cannot write them\n", n_gpus);

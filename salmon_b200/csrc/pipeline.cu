@@ -365,6 +365,7 @@ struct MetaIn {
   int n_ranks;
   uint64_t lib_counts[4];     // fragments that showed ISF / ISR / SF / SR among their kept mappings
   uint64_t orphans_rescued;   // over all ranks
+  uint64_t n_compatible;      // assigned fragments with a kept mapping compatible with the library type, over all ranks
 };
 std::string time_string() {
   time_t t = time(nullptr);
@@ -410,7 +411,7 @@ int write_run_metadata(const std::string& outs, const MetaIn& m) {
     for (int i = 0; i < 10000; ++i) ++samples[dist(gen)];
   }
   bool ok = write_gz(outs + "/aux_info/fld.gz", samples.data(), samples.size() * 4);
-  {   // libParams/flenDist.txt: exp(pmf(i)), tab separated, ostream precision
+  if (!m.mp->no_frag_len_dist) {   // libParams/flenDist.txt: exp(pmf(i)), tab separated, ostream precision
     std::string t;
     char buf[48];
     for (size_t i = 0; i < pmf.size(); ++i) { snprintf(buf, sizeof buf, "%g", pmf[i]); t += buf; t += (i + 1 < pmf.size()) ? "\t" : "\n"; }
@@ -447,9 +448,10 @@ int write_run_metadata(const std::string& outs, const MetaIn& m) {
              (unsigned long long)m.orphans_rescued);
     ok = write_text(outs + "/aux_info/meta_info.json", buf) && ok;
   }
-  {   // lib_format_counts.json (ReadExperiment.inl:219-350): every kept mapping is compatible with the expected format
-      // (incompatible ones are ignored while mapping), so compatible = assigned; the per-format counts are what the
-      // fragments showed; strand_mapping_bias = first strand variant / both, as summarizeLibraryTypeCounts computes it
+  {   // lib_format_counts.json (ReadExperiment.inl:219-350): compatible = assigned fragments with at least one kept mapping
+      // compatible with the expected format (all of them unless --incompatPrior keeps incompatible ones); the per-format
+      // counts are what the fragments showed; strand_mapping_bias = first strand variant / both, as
+      // summarizeLibraryTypeCounts computes it
     static const char* const lib_names[] = {"IU", "ISF", "ISR", "U", "SF", "SR"};
     const int lt = m.mp->lib_type;
     const bool pe = lt < 3;
@@ -464,7 +466,8 @@ int write_run_metadata(const std::string& outs, const MetaIn& m) {
              "    \"num_compatible_fragments\": %llu,\n    \"num_assigned_fragments\": %llu,\n"
              "    \"num_frags_with_concordant_consistent_mappings\": %llu,\n    \"num_frags_with_inconsistent_or_orphan_mappings\": %llu,\n"
              "    \"strand_mapping_bias\": %.6f,\n    \"ISF\": %llu,\n    \"ISR\": %llu,\n    \"SF\": %llu,\n    \"SR\": %llu\n}\n",
-             m.files.c_str(), lib_names[lt < 0 || lt > 5 ? 0 : lt], m.n_mapped ? 1.0 : 0.0, (unsigned long long)m.n_mapped,
+             m.files.c_str(), lib_names[lt < 0 || lt > 5 ? 0 : lt],
+             m.n_mapped ? (double)m.n_compatible / (double)m.n_mapped : 0.0, (unsigned long long)m.n_compatible,
              (unsigned long long)m.n_mapped, (unsigned long long)agree, (unsigned long long)other, ratio,
              (unsigned long long)m.lib_counts[0], (unsigned long long)m.lib_counts[1], (unsigned long long)m.lib_counts[2],
              (unsigned long long)m.lib_counts[3]);
@@ -735,7 +738,7 @@ extern "C" int sb_quant_files(sb_index* ix, const char* const* mates1, const cha
   // (a collective: every rank takes part, whether it writes the outputs or not)
   uint64_t libc[5] = {res.lib_format_counts[0], res.lib_format_counts[1], res.lib_format_counts[2], res.lib_format_counts[3],
                       res.orphans_rescued};
-  if (multi) SB_TRY(sb_comm_allreduce(S.comm, libc, 5, 1, 0));
+  if (multi) SB_TRY(sb_comm_allreduce(S.comm, libc, 5, 1, 0));   // (glob.n_compatible is global already)
   if (!outs.empty() && o.shard_index == 0) {
     if (!make_dirs(outs + "/aux_info")) { sb::set_error("cannot create %s/aux_info", outs.c_str()); return SB_ERR_INVALID; }
     std::vector<uint32_t> lens;
@@ -758,7 +761,8 @@ extern "C" int sb_quant_files(sb_index* ix, const char* const* mates1, const cha
       files += std::string(f ? ", " : "") + (mates2 ? std::string("( ") + mates1[f] + ", " + mates2[f] + " )" : std::string(mates1[f]));
     files += " ]";
     MetaIn mi{&o, &ep, &mp, Mq, M - Mq, n_observed, n_mapped_u, res.n_classes, &hist, glob.unique_counts, glob.total_counts,
-              files, start_time, time_string(), (int)o.shard_count, {libc[0], libc[1], libc[2], libc[3]}, libc[4]};
+              files, start_time, time_string(), (int)o.shard_count, {libc[0], libc[1], libc[2], libc[3]}, libc[4],
+              glob.n_compatible};
     SB_TRY(write_run_metadata(outs, mi));
   }
   if (o.num_bootstraps || o.num_gibbs) {
@@ -853,6 +857,7 @@ extern "C" int sb_map_reduce_global(sb_map_ctx* ctx, sb_comm* comm, sb_map_resul
   const uint32_t M = p.n_txps, nf = p.n_fld;
   if (G == 1) {
     if (assigned_out) *assigned_out = p.assigned;
+    out->n_compatible = p.compatible;
     return sb_map_project_global(ctx, &p, 1, p.cluster_root, out);
   }
   // log-sum-exp over the ranks; +inf = no mass (salmon's LOG_0); `prior` (counted by every rank) is kept once
@@ -884,15 +889,16 @@ extern "C" int sb_map_reduce_global(sb_map_ctx* ctx, sb_comm* comm, sb_map_resul
   SB_TRY(sb_comm_allreduce(comm, uniq.data(), M, 1, 0));
   SB_TRY(sb_comm_allreduce(comm, total.data(), M, 1, 0));
   SB_TRY(sb_comm_allreduce(comm, hits.data(), M, 1, 0));
-  uint64_t scal[2] = {p.fld_min, p.assigned};
+  uint64_t scal[3] = {p.fld_min, p.assigned, p.compatible};
   SB_TRY(sb_comm_allreduce(comm, &scal[0], 1, 1, 3));
-  SB_TRY(sb_comm_allreduce(comm, &scal[1], 1, 1, 0));
+  SB_TRY(sb_comm_allreduce(comm, &scal[1], 2, 1, 0));
   std::vector<uint32_t> roots((size_t)G * std::max<uint32_t>(M, 1));
   SB_TRY(sb_comm_allgather(comm, p.cluster_root, roots.data(), (size_t)M * 4));
   sb_map_partial g = p;
   g.mass = mass.data(); g.fld_hist = hist.data(); g.fld_tot = tot1[0];
   g.unique_counts = uniq.data(); g.total_counts = total.data(); g.cluster_hits = hits.data();
-  g.fld_min = (uint32_t)scal[0]; g.assigned = scal[1];
+  g.fld_min = (uint32_t)scal[0]; g.assigned = scal[1]; g.compatible = scal[2];
   if (assigned_out) *assigned_out = scal[1];
+  out->n_compatible = scal[2];
   return sb_map_project_global(ctx, &g, (uint32_t)G, roots.data(), out);
 }

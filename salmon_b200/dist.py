@@ -53,6 +53,7 @@ def reduce_partials(p: dict, dist=None, device="cpu"):
         g[k] = allreduce(p[k].astype(np.int64), dist.ReduceOp.SUM).astype(np.uint64)
     g["fld_min"] = int(allreduce(np.array([p["fld_min"]], dtype=np.int64), dist.ReduceOp.MIN)[0])
     g["assigned"] = int(allreduce(np.array([p["assigned"]], dtype=np.int64), dist.ReduceOp.SUM)[0])
+    g["compatible"] = int(allreduce(np.array([p.get("compatible", 0)], dtype=np.int64), dist.ReduceOp.SUM)[0])
     mine = _t(p["cluster_root"].astype(np.int64), device)
     parts = [torch.empty_like(mine) for _ in range(world)]
     dist.all_gather(parts, mine)

@@ -27,6 +27,20 @@ def _boot_params(ep):
     return bp
 
 
+def _likelihood_options(mp, incompat_prior, no_single_frag_prob, no_frag_len_dist, no_eff_len_correction):
+    """salmon's fragment-likelihood options on map_params (DESIGN.md section 13); the defaults leave mp as it is"""
+    if incompat_prior:
+        p = float(incompat_prior)
+        mp.incompat_prior = 0.0 if p < 1e-100 else p     # below 1e-100: incompatible mappings are ignored
+    if no_single_frag_prob:
+        mp.no_single_frag_prob = 1
+    if no_frag_len_dist:
+        mp.no_frag_len_dist = 1
+    if no_eff_len_correction:
+        mp.no_eff_len_correction = 1
+    return mp
+
+
 def _drop_decoys(index, inputs):
     """readExp.dropDecoyTranscripts() (SalmonQuantify.cpp:2479, ReadExperiment.hpp:120): decoys -- the suffix of the id
     space, never part of a label -- leave before the optimiser and the writers.  Returns (Mq, inputs cut to Mq)."""
@@ -43,10 +57,14 @@ def _drop_decoys(index, inputs):
 
 
 def quant_reads(index, left, right, map_params=None, em_params=None, device=0, batch=262_144, dist=None,
-                names=None, out_dir=None, dump_eq=False, dump_eq_weights=False):
-    """left/right: [n, L] uint8 base codes (0..3 = ACGT, 4 = N) of THIS rank's read shard.
+                names=None, out_dir=None, dump_eq=False, dump_eq_weights=False, incompat_prior=0.0,
+                no_single_frag_prob=False, no_frag_len_dist=False, no_eff_len_correction=False):
+    """left/right: [n, L] uint8 base codes (0..3 = ACGT, 4 = N) of THIS rank's read shard.  incompat_prior,
+    no_single_frag_prob, no_frag_len_dist, no_eff_len_correction: `--incompatPrior`, `--noSingleFragProb`,
+    `--noFragLengthDist`, `--noEffectiveLengthCorrection` (set on map_params; DESIGN.md section 13).
     Returns dict(alpha, tpm, eff_len, classes, n_mapped, em_stats)."""
-    mp = map_params or map_default_params()
+    mp = _likelihood_options(map_params or map_default_params(), incompat_prior, no_single_frag_prob, no_frag_len_dist,
+                             no_eff_len_correction)
     ep = em_params or default_params()
     n, L = left.shape
     world = dist.get_world_size() if (dist is not None and dist.is_initialized()) else 1
@@ -143,7 +161,8 @@ def _quantify(index, ctx, ep, device, dist, names, out_dir, dump_eq, dump_eq_wei
 def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=None, device=0, batch=262_144,
                 max_read_len=256, threads=8, dist=None, dump_eq=False, dump_eq_weights=False, num_bootstraps=0, seed=0,
                 write_mappings=None, write_qualities=False, write_unmapped_names=False, cmdline="", recover_orphans=False,
-                softclip=0):
+                softclip=0, incompat_prior=0.0, no_single_frag_prob=False, no_frag_len_dist=False,
+                no_eff_len_correction=False):
     """`salmon quant -i index -l IU -1 mates1 -2 mates2 -o out_dir` for the hot path: FASTQ/FASTA(.gz) files ->
     sb_reads_bucketed -> sb_map_batch -> ... -> quant.sf.  index: an _capi.Index or the path of a saved one.  With
     torch.distributed initialised every rank takes the global batches g with g % world == rank (round-robin sharding
@@ -153,7 +172,9 @@ def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=
     qualities when write_qualities; write_unmapped_names: out_dir/aux_info/unmapped_names.txt.  Both need one GPU.
     recover_orphans: `--recoverOrphans` (sets map_params.recover_orphans; single-end reads: no effect).
     softclip: scoring mode of the DP (sets map_params.softclip when non-zero): 1 = `--softclipOverhangs`, 2 =
-    `--softclip` (DESIGN.md section 12)."""
+    `--softclip` (DESIGN.md section 12).  incompat_prior, no_single_frag_prob, no_frag_len_dist, no_eff_len_correction:
+    `--incompatPrior`, `--noSingleFragProb`, `--noFragLengthDist`, `--noEffectiveLengthCorrection` (DESIGN.md section
+    13)."""
     if isinstance(index, (str, bytes, os.PathLike)):
         index = _capi.Index.load(index)
     mp = map_params or map_default_params()
@@ -161,6 +182,7 @@ def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=
         mp.recover_orphans = 1
     if softclip:
         mp.softclip = int(softclip)
+    _likelihood_options(mp, incompat_prior, no_single_frag_prob, no_frag_len_dist, no_eff_len_correction)
     meta = index.meta()
     if meta["first_decoy"] < index.n_txps:
         mp.first_decoy = meta["first_decoy"]

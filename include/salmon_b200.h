@@ -627,11 +627,9 @@ int sb_em_debug_timeline(sb_em_ctx* ctx, uint64_t* out, uint32_t iteration);
 
 /* Tuning knobs (not part of the reference contract).  Unknown keys return SB_ERR_INVALID.
  * key: "variant" (0 = multi-kernel per iteration, 1 = persistent cooperative), "blocks_per_sm" (0 = as many as fit),
- *      "config" (kernel configuration 0-3: ring chunk x depth x resident blocks), "lmax" (longest row on the SELL path),
- *      "lwarp" (longest row reduced by one warp), "sell_group_cm" / "sell_group_tm" (rows per length-bucketing group, a
- *      power of two >= 32), "rebalance" (rounds of measured re-cutting of the warp ranges), "rebalance_iters",
- *      "overhead_p1" / "overhead_p2" (per-slice epilogue cost in columns, for the range cut), "push_pass" (fused
- *      multi-GPU path: -1 by rank count, 0 push from the row epilogues, 1 coalesced pass), "sample_offset". */
+ *      "sell_group_cm" / "sell_group_tm" (rows per length-bucketing group, a power of two >= 32), "rebalance" (rounds
+ *      of measured re-cutting of the warp ranges), "push_pass" (fused multi-GPU path: -1 by rank count, 0 push from the
+ *      row epilogues, 1 coalesced pass), "sample_offset". */
 int sb_em_set_option(sb_em_ctx* ctx, const char* key, int64_t value);
 
 /* Figures of the layout sb_em_prepare built (after prepare).  key: "stream_bytes" (bytes one iteration streams:

@@ -34,51 +34,15 @@
 namespace sb {
 
 // ---------------------------------------------------------------------------
-// kernel configurations: ring chunk (columns) x resident blocks per SM
+// the iteration kernels: [0] = plain EM, [1] = VBEM (compile-time variants: the NaN guard exists in EM only, the
+// digamma/exp epilogue in VBEM only).  Every one takes EM_SMEM bytes of dynamic shared memory.
 // ---------------------------------------------------------------------------
-struct KernelSet {
-  const char* name;
-  int ch, ring;      // ring chunk (columns) x chunks in flight per warp
-  size_t smem;
-  // [0] = plain EM, [1] = VBEM (compile-time variants: the NaN guard exists in EM only, the digamma/exp epilogue in VBEM only)
-  const void* persistent[2];
-  const void* persistent_mgpu[2];
-  void (*p1[2])(EmArgs);
-  void (*p2[2])(EmArgs, uint32_t);
-  void (*p2_partial[2])(EmArgs);
-};
-template <int CH, int RING, int MINB>
-static KernelSet make_set(const char* name) {
-  KernelSet k;
-  k.name = name;
-  k.ch = CH;
-  k.ring = RING;
-  k.smem = em_smem<CH, RING>();
-  k.persistent[0] = (const void*)k_em_persistent<CH, RING, MINB, false>;
-  k.persistent[1] = (const void*)k_em_persistent<CH, RING, MINB, true>;
-  k.persistent_mgpu[0] = (const void*)k_em_persistent_mgpu<CH, RING, MINB, false>;
-  k.persistent_mgpu[1] = (const void*)k_em_persistent_mgpu<CH, RING, MINB, true>;
-  k.p1[0] = k_em_p1<CH, RING, MINB, false>;
-  k.p1[1] = k_em_p1<CH, RING, MINB, true>;
-  k.p2[0] = k_em_p2<CH, RING, MINB, false>;
-  k.p2[1] = k_em_p2<CH, RING, MINB, true>;
-  k.p2_partial[0] = k_em_p2_partial<CH, RING, MINB, false>;
-  k.p2_partial[1] = k_em_p2_partial<CH, RING, MINB, true>;
-  return k;
-}
-// chunk columns x ring depth x resident blocks per SM (shared memory per block = 8 warps x CH x RING x 320 B, a column
-// being 32 x (2-byte index + 8-byte weight)):
-//   0: 16x2 b2 (80 KB, 16 warps/SM)   1: 8x4 b2 (80 KB)   2: 8x3 b3 (60 KB, 24 warps/SM)   3: 8x2 b4 (40 KB, 32 warps/SM)
-// (the resident blocks are capped by the registers the launch bounds allow, not by the shared memory)
-constexpr int N_KERNEL_SETS = 4;
-static const KernelSet& kernel_set(int cfg) {
-  static const KernelSet sets[N_KERNEL_SETS] = {
-      make_set<16, 2, 2>("ch16r2b2"), make_set<8, 4, 2>("ch8r4b2"), make_set<8, 3, 3>("ch8r3b3"),
-      make_set<8, 2, 4>("ch8r2b4"),
-  };
-  if (cfg < 0 || cfg >= N_KERNEL_SETS) cfg = 0;
-  return sets[cfg];
-}
+static const void* const K_PERSISTENT[2] = {(const void*)k_em_persistent<false>, (const void*)k_em_persistent<true>};
+static const void* const K_PERSISTENT_MGPU[2] = {(const void*)k_em_persistent_mgpu<false>,
+                                                 (const void*)k_em_persistent_mgpu<true>};
+static void (*const K_P1[2])(EmArgs) = {k_em_p1<false>, k_em_p1<true>};
+static void (*const K_P2[2])(EmArgs, uint32_t) = {k_em_p2<false>, k_em_p2<true>};
+static void (*const K_P2_PARTIAL[2])(EmArgs) = {k_em_p2_partial<false>, k_em_p2_partial<true>};
 
 // ---------------------------------------------------------------------------
 // prepare kernels
@@ -272,8 +236,7 @@ __global__ void k_remap(uint32_t n, const uint32_t* __restrict__ src,
 // one warp per slice: row lengths, slice width (= max non-long length, exact), base index (= smallest gather index of
 // its SELL rows).  A slice whose indices do not fit 16 bits relative to the base (IDX_PAD is reserved) sends its rows
 // to the long-row path (counts: [0] long rows, [2] of which fallback rows).
-__global__ void k_sell_widths(uint32_t n_rows, uint32_t n_slices, uint32_t lmax,
-                              const uint32_t* __restrict__ rowperm,
+__global__ void k_sell_widths(uint32_t n_rows, uint32_t n_slices, const uint32_t* __restrict__ rowperm,
                               const uint32_t* __restrict__ csr_off, const uint32_t* __restrict__ csr_idx,
                               uint16_t* __restrict__ len16, uint32_t* __restrict__ width,
                               uint32_t* __restrict__ sbase, uint32_t* __restrict__ counts) {
@@ -287,7 +250,7 @@ __global__ void k_sell_widths(uint32_t n_rows, uint32_t n_slices, uint32_t lmax,
     const uint32_t cr = rowperm ? rowperm[row] : row;
     const uint32_t b = csr_off[cr];
     len = csr_off[cr + 1] - b;
-    sell = len <= lmax;
+    sell = len <= LMAX;
     if (!sell) {
       len16[row] = LEN_LONG;
       atomicAdd(&counts[0], 1u);
@@ -542,8 +505,6 @@ extern "C" sb_em_ctx* sb_em_create(int device) {
   c->l2_bytes = (size_t)prop.l2CacheSize;
   for (int i = 0; i < 4; ++i) cudaEventCreate(&c->ev[i]);
   // development overrides of the tuning defaults (sweeps over the test-suite)
-  if (const char* e = getenv("SB_EM_CONFIG")) { const int v = atoi(e); if (v >= 0 && v < N_KERNEL_SETS) c->config = v; }
-  if (const char* e = getenv("SB_EM_LWARP")) { const int v = atoi(e); if (v >= 1) c->lwarp = v; }
   if (const char* e = getenv("SB_EM_GROUP_CM")) { const int v = atoi(e); if (v >= 32 && !(v & (v - 1))) c->sell_group_cm = v; }
   if (const char* e = getenv("SB_EM_GROUP_TM")) { const int v = atoi(e); if (v >= 32 && !(v & (v - 1))) c->sell_group_tm = v; }
   return c;
@@ -605,26 +566,13 @@ extern "C" int sb_em_set_option(sb_em_ctx* c, const char* key, int64_t value) {
   if (!c || !key) { set_error("null argument"); return SB_ERR_INVALID; }
   if (!strcmp(key, "variant")) c->variant = (int)value;
   else if (!strcmp(key, "blocks_per_sm")) { c->blocks_per_sm = (int)value; c->prepared = false; }
-  else if (!strcmp(key, "config")) {
-    if (value < 0 || value >= N_KERNEL_SETS) { set_error("config out of range"); return SB_ERR_INVALID; }
-    c->config = (int)value;
-    c->prepared = false;
-  } else if (!strcmp(key, "lmax")) {
-    if (value < 1 || value > 60000) { set_error("lmax out of range"); return SB_ERR_INVALID; }
-    c->lmax = (int)value; c->prepared = false;
-  } else if (!strcmp(key, "sell_group_cm") || !strcmp(key, "sell_group_tm")) {
+  else if (!strcmp(key, "sell_group_cm") || !strcmp(key, "sell_group_tm")) {
     if (value < 32 || value > (1 << 20) || (value & (value - 1))) { set_error("sell_group must be a power of two >= 32"); return SB_ERR_INVALID; }
     (key[11] == 'c' ? c->sell_group_cm : c->sell_group_tm) = (int)value; c->prepared = false;
-  } else if (!strcmp(key, "lwarp")) {
-    if (value < 1 || value > 1000000) { set_error("lwarp out of range"); return SB_ERR_INVALID; }
-    c->lwarp = (int)value; c->prepared = false;
   }
   else if (!strcmp(key, "push_pass")) { c->push_pass = (int)value; }
   else if (!strcmp(key, "sample_offset")) { c->sample_offset = (uint32_t)value; }
   else if (!strcmp(key, "rebalance")) { c->rebalance = (int)value; c->prepared = false; }
-  else if (!strcmp(key, "rebalance_iters")) { c->rebalance_iters = (int)value; c->prepared = false; }
-  else if (!strcmp(key, "overhead_p1")) { c->ovh_p1 = (int)value; c->prepared = false; }
-  else if (!strcmp(key, "overhead_p2")) { c->ovh_p2 = (int)value; c->prepared = false; }
   else { set_error("unknown option '%s'", key); return SB_ERR_INVALID; }
   return SB_OK;
 }
@@ -638,11 +586,7 @@ extern "C" int sb_em_get_info(sb_em_ctx* c, const char* key, int64_t* value) {
   if (!strcmp(key, "stream_bytes")) { *value = stream(c->cm) + stream(c->tm); return SB_OK; }
   // warps of the grid the slice ranges were cut for, and the columns one warp's ring holds
   if (!strcmp(key, "warps")) { *value = (int64_t)c->grid * (EM_THREADS / 32); return SB_OK; }
-  if (!strcmp(key, "ring_cols")) {
-    const KernelSet& ks = kernel_set(c->config);
-    *value = (int64_t)ks.ch * ks.ring;
-    return SB_OK;
-  }
+  if (!strcmp(key, "ring_cols")) { *value = (int64_t)EM_CH * EM_RING; return SB_OK; }
   const size_t n = strlen(key);
   const SellDev* m = nullptr;
   if (n > 3 && !strcmp(key + n - 3, "_cm")) m = &c->cm;
@@ -730,6 +674,10 @@ static int scan_u64(sb_em_ctx* c, const uint64_t* in, uint64_t* out, uint64_t n)
   return SB_OK;
 }
 
+// epilogue overhead of a slice in columns, for cutting the warp ranges: P1 (and plain EM's P2), VBEM's P2
+constexpr uint32_t OVERHEAD_P1 = 3, OVERHEAD_P2 = 12;
+static uint32_t overhead_tm(const sb_em_ctx* c) { return c->params.use_vbem ? OVERHEAD_P2 : OVERHEAD_P1; }
+
 // modelled cost of a slice in columns: its width plus the epilogue overhead (slices of long rows only cost nothing)
 static double slice_cost(const std::vector<uint32_t>& sp, uint32_t s, uint32_t overhead) {
   return (double)(sp[s + 1] - sp[s]) + (sp[s + 1] > sp[s] ? (double)overhead : 0.0);
@@ -754,8 +702,8 @@ static int build_sell(sb_em_ctx* c, SellDev& m, uint32_t n_rows, const uint32_t*
   SB_CUDA(cudaMemsetAsync(d_nlong, 0, 16, st));
   SB_CUDA(cudaMemsetAsync(m.width, 0, ((size_t)m.n_slices + 1) * 4, st));
   if (m.n_slices) {
-    k_sell_widths<<<nblk(m.n_slices, 8), 256, 0, st>>>(n_rows, m.n_slices, (uint32_t)c->lmax, rowperm, csr_off, csr_idx,
-                                                       m.len, m.width, m.base, d_nlong);
+    k_sell_widths<<<nblk(m.n_slices, 8), 256, 0, st>>>(n_rows, m.n_slices, rowperm, csr_off, csr_idx, m.len, m.width,
+                                                       m.base, d_nlong);
     c->launches++;
   }
   {
@@ -796,7 +744,7 @@ static int build_sell(sb_em_ctx* c, SellDev& m, uint32_t n_rows, const uint32_t*
       return lx != ly ? lx > ly : h[3 * x] < h[3 * y];
     });
     for (uint32_t i = 0; i < m.n_long; ++i) {
-      if (h[3 * ord[i] + 2] - h[3 * ord[i] + 1] > (uint32_t)c->lwarp) m.n_block = i + 1;
+      if (h[3 * ord[i] + 2] - h[3 * ord[i] + 1] > LWARP) m.n_block = i + 1;
       m.long_entries += h[3 * i + 2] - h[3 * i + 1];
     }
     std::vector<uint32_t> h2(h.size());
@@ -827,17 +775,16 @@ extern "C" int sb_em_prepare(sb_em_ctx* c, const sb_em_params* p, sb_em_stats* s
 
   // launch geometry first: the slice ranges are cut for this grid
   int occ = 0;
-  const KernelSet& ks = kernel_set(c->config);
   for (int v = 0; v < 2; ++v) {
-    SB_CUDA(cudaFuncSetAttribute(ks.persistent[v], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ks.smem));
-    SB_CUDA(cudaFuncSetAttribute((const void*)ks.p1[v], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ks.smem));
-    SB_CUDA(cudaFuncSetAttribute((const void*)ks.p2[v], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ks.smem));
-    SB_CUDA(cudaFuncSetAttribute((const void*)ks.p2_partial[v], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ks.smem));
-    SB_CUDA(cudaFuncSetAttribute(ks.persistent_mgpu[v], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ks.smem));
+    SB_CUDA(cudaFuncSetAttribute(K_PERSISTENT[v], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EM_SMEM));
+    SB_CUDA(cudaFuncSetAttribute((const void*)K_P1[v], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EM_SMEM));
+    SB_CUDA(cudaFuncSetAttribute((const void*)K_P2[v], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EM_SMEM));
+    SB_CUDA(cudaFuncSetAttribute((const void*)K_P2_PARTIAL[v], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EM_SMEM));
+    SB_CUDA(cudaFuncSetAttribute(K_PERSISTENT_MGPU[v], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EM_SMEM));
   }
   const int vb = p->use_vbem ? 1 : 0;
-  SB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (c->nranks > 1 || c->fused_loopback) ? ks.persistent_mgpu[vb] : ks.persistent[vb],
-                                                        EM_THREADS, ks.smem));
+  SB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (c->nranks > 1 || c->fused_loopback) ? K_PERSISTENT_MGPU[vb] : K_PERSISTENT[vb],
+                                                        EM_THREADS, EM_SMEM));
   if (occ < 1) { set_error("persistent EM kernel does not fit on an SM"); return SB_ERR_CUDA; }
   if (c->blocks_per_sm > 0) occ = std::min(occ, c->blocks_per_sm);
   c->grid = (uint32_t)(occ * c->n_sm);
@@ -996,9 +943,8 @@ extern "C" int sb_em_prepare(sb_em_ctx* c, const sb_em_params* p, sb_em_stats* s
     }
   }
   // SELL-32 copies.  overhead = per-slice epilogue cost in "columns" for the work split
-  SB_TRY(build_sell(c, c->cm, Cm, nullptr, c->m_off, c->m_idx_state, c->m_w, row_space ? R : M, (uint32_t)c->ovh_p1, n_warps));
-  SB_TRY(build_sell(c, c->tm, R, c->d_rowperm, c->t_off, c->t_idx, c->t_w, Cm,
-                    (uint32_t)(c->params.use_vbem ? c->ovh_p2 : c->ovh_p1), n_warps));
+  SB_TRY(build_sell(c, c->cm, Cm, nullptr, c->m_off, c->m_idx_state, c->m_w, row_space ? R : M, OVERHEAD_P1, n_warps));
+  SB_TRY(build_sell(c, c->tm, R, c->d_rowperm, c->t_off, c->t_idx, c->t_w, Cm, overhead_tm(c), n_warps));
 
   // iteration-0 reductions
   double* d_sum0 = c->d_scalars + 16;
@@ -1289,7 +1235,7 @@ extern "C" int sb_em_peer_open(sb_em_ctx* c, int rank, int nranks, const void* h
 
 // Fused path: one cooperative launch per run on every rank; the partial alpha' are pushed to their owners, the owners
 // push theta back, all inside the kernel over the peers' exchange blocks (see k_em_persistent_mgpu).
-static int em_run_multi_gpu_fused(sb_em_ctx* c, const KernelSet& ks, EmArgs& A, uint32_t* out,
+static int em_run_multi_gpu_fused(sb_em_ctx* c, EmArgs& A, uint32_t* out,
                                   uint32_t* launches, uint32_t* loop_launches, float* loop_ms) {
   cudaStream_t st = c->stream;
   const uint32_t M = c->M;
@@ -1308,7 +1254,7 @@ static int em_run_multi_gpu_fused(sb_em_ctx* c, const KernelSet& ks, EmArgs& A, 
   A.epoch0 = c->x_epoch; A.xfail = c->d_xfail;
   void* args[] = {(void*)&A};
   SB_CUDA(cudaEventRecord(c->ev[2], st));
-  SB_CUDA(cudaLaunchCooperativeKernel(ks.persistent_mgpu[vb], dim3(c->grid), dim3(EM_THREADS), args, ks.smem, st));
+  SB_CUDA(cudaLaunchCooperativeKernel(K_PERSISTENT_MGPU[vb], dim3(c->grid), dim3(EM_THREADS), args, EM_SMEM, st));
   SB_CUDA(cudaEventRecord(c->ev[3], st));
   *launches += 1; *loop_launches += 1;
   uint32_t fail = 0;
@@ -1323,7 +1269,7 @@ static int em_run_multi_gpu_fused(sb_em_ctx* c, const KernelSet& ks, EmArgs& A, 
 }
 
 // One iteration = P1, P2-partial, all-reduce(alpha'), update.  Classes stay sharded.
-static int em_run_multi_gpu(sb_em_ctx* c, const KernelSet& ks, EmArgs& A, uint32_t* out,
+static int em_run_multi_gpu(sb_em_ctx* c, EmArgs& A, uint32_t* out,
                             uint32_t* launches, uint32_t* loop_launches, float* loop_ms) {
   cudaStream_t st = c->stream;
   const uint32_t M = c->M;
@@ -1341,8 +1287,8 @@ static int em_run_multi_gpu(sb_em_ctx* c, const KernelSet& ks, EmArgs& A, uint32
   SB_CUDA(cudaEventRecord(c->ev[2], st));
   while (it < A.min_iter || (it < A.max_iter && !converged)) {
     k_reset_maxrel<<<1, 1, 0, st>>>(A.maxrel, it & 1u);
-    ks.p1[vb]<<<c->grid, EM_THREADS, ks.smem, st>>>(A);
-    ks.p2_partial[vb]<<<c->grid, EM_THREADS, ks.smem, st>>>(A);
+    K_P1[vb]<<<c->grid, EM_THREADS, EM_SMEM, st>>>(A);
+    K_P2_PARTIAL[vb]<<<c->grid, EM_THREADS, EM_SMEM, st>>>(A);
     SB_NCCL(g_nccl.AllReduce(c->d_part, c->d_part_red, (size_t)M, /*ncclFloat64*/ 8, /*ncclSum*/ 0,
                              c->nccl_comm, st));
     if (vb) k_em_update<true><<<ugrid, 256, 0, st>>>(A, c->d_part_red, M, it);
@@ -1370,7 +1316,6 @@ extern "C" int sb_em_run(sb_em_ctx* c, sb_em_stats* stats) {
   if (!c->prepared) { set_error("sb_em_run before sb_em_prepare"); return SB_ERR_STATE; }
   SB_CUDA(cudaSetDevice(c->device));
   cudaStream_t st = c->stream;
-  const KernelSet& ks = kernel_set(c->config);
   const uint32_t M = c->M;
   const uint32_t R = c->n_rows;
   const bool multi_gpu = c->nranks > 1 || c->fused_loopback;
@@ -1404,13 +1349,13 @@ extern "C" int sb_em_run(sb_em_ctx* c, sb_em_stats* stats) {
   if (c->params.max_iter == 0 && c->params.min_iter == 0) {
     // nothing to iterate
   } else if (multi_gpu) {
-    int r = fused ? em_run_multi_gpu_fused(c, ks, A, out, &launches, &loop_launches, &loop_ms)
-                  : em_run_multi_gpu(c, ks, A, out, &launches, &loop_launches, &loop_ms);
+    int r = fused ? em_run_multi_gpu_fused(c, A, out, &launches, &loop_launches, &loop_ms)
+                  : em_run_multi_gpu(c, A, out, &launches, &loop_launches, &loop_ms);
     if (r != SB_OK) return r;
   } else if (c->variant == 1) {
     void* args[] = {(void*)&A};
     SB_CUDA(cudaEventRecord(c->ev[2], st));
-    SB_CUDA(cudaLaunchCooperativeKernel(ks.persistent[vb], dim3(c->grid), dim3(EM_THREADS), args, ks.smem, st));
+    SB_CUDA(cudaLaunchCooperativeKernel(K_PERSISTENT[vb], dim3(c->grid), dim3(EM_THREADS), args, EM_SMEM, st));
     SB_CUDA(cudaEventRecord(c->ev[3], st));
     ++launches; ++loop_launches;
     SB_CUDA(cudaMemcpyAsync(out, A.out, 16, cudaMemcpyDeviceToHost, st));
@@ -1424,8 +1369,8 @@ extern "C" int sb_em_run(sb_em_ctx* c, sb_em_stats* stats) {
     SB_CUDA(cudaEventRecord(c->ev[2], st));
     while (it < A.min_iter || (it < A.max_iter && !converged)) {
       k_reset_maxrel<<<1, 1, 0, st>>>(A.maxrel, it & 1u);
-      ks.p1[vb]<<<c->grid, EM_THREADS, ks.smem, st>>>(A);
-      ks.p2[vb]<<<c->grid, EM_THREADS, ks.smem, st>>>(A, it);
+      K_P1[vb]<<<c->grid, EM_THREADS, EM_SMEM, st>>>(A);
+      K_P2[vb]<<<c->grid, EM_THREADS, EM_SMEM, st>>>(A, it);
       launches += 3; loop_launches += 2;
       ++it;
       if (it >= A.min_iter) {
@@ -1538,6 +1483,8 @@ static int em_recut(sb::SellDev& m, uint32_t overhead, const std::vector<unsigne
   return SB_OK;
 }
 
+constexpr uint32_t REBALANCE_ITERS = 8;   // measured iterations of the instrumented run (the first is not timed)
+
 static int em_rebalance(sb_em_ctx* c) {
   const uint32_t n_warps = c->grid * (EM_THREADS / 32);
   SB_TRY(dev_alloc(&c->d_dbg, (size_t)n_warps * DBG_SLOTS));
@@ -1545,7 +1492,7 @@ static int em_rebalance(sb_em_ctx* c) {
   const sb_em_params saved = c->params;
   const uint32_t saved_it = c->dbg_it;
   const bool saved_en = c->dbg_enabled;
-  c->params.min_iter = c->params.max_iter = (uint32_t)std::max(2, c->rebalance_iters + 1);
+  c->params.min_iter = c->params.max_iter = REBALANCE_ITERS + 1;
   c->dbg_it = DBG_ACCUMULATE;
   c->dbg_enabled = true;
   int rc = sb_em_run(c, nullptr);
@@ -1553,9 +1500,8 @@ static int em_rebalance(sb_em_ctx* c) {
   if (rc != SB_OK) return rc;
   std::vector<unsigned long long> dbg((size_t)n_warps * DBG_SLOTS);
   SB_CUDA(cudaMemcpy(dbg.data(), c->d_dbg, dbg.size() * 8, cudaMemcpyDeviceToHost));
-  const uint32_t ovh_tm = (uint32_t)(c->params.use_vbem ? c->ovh_p2 : c->ovh_p1);
-  SB_TRY(em_recut(c->cm, (uint32_t)c->ovh_p1, dbg, 0, 3, n_warps));
-  SB_TRY(em_recut(c->tm, ovh_tm, dbg, 1, 4, n_warps));
+  SB_TRY(em_recut(c->cm, OVERHEAD_P1, dbg, 0, 3, n_warps));
+  SB_TRY(em_recut(c->tm, overhead_tm(c), dbg, 1, 4, n_warps));
   return SB_OK;
 }
 

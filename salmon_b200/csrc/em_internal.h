@@ -9,6 +9,8 @@
 
 namespace sb {
 
+constexpr int SELL_GROUP = 1024;    // default rows per length-bucketing group (options sell_group_cm / sell_group_tm)
+
 // Device-side owner of one SELL-32 matrix (see em_kernels.cuh: struct Sell).
 struct SellDev {
   uint32_t n_rows = 0, n_slices = 0, n_cols = 0, n_long = 0, n_block = 0;
@@ -39,14 +41,10 @@ struct sb_em_ctx {
   // options
   int variant = 1;        // 1 = persistent cooperative kernel, 0 = one launch per phase
   int blocks_per_sm = 0;  // 0 = as many as fit
-  int config = 1;         // kernel configuration (ring chunk x depth x resident blocks), see kernel_set(); 8x4 b2 is the fastest on H100
   int rebalance = 1;      // rounds of measured re-cutting of the warp ranges at prepare (0 = column-count model only)
-  int rebalance_iters = 8;
   int occ = 0;
-  int ovh_p1 = 3, ovh_p2 = 12;
-  int lmax = 96;                    // longest row kept on the lane-per-row SELL path
-  int sell_group_cm = 1024, sell_group_tm = 1024;   // rows per length-bucketing group (locality window of the gathers)
-  int lwarp = 2048;                 // longest row reduced by one warp (longer: one block)
+  // rows per length-bucketing group (locality window of the gathers)
+  int sell_group_cm = sb::SELL_GROUP, sell_group_tm = sb::SELL_GROUP;
 
   // problem
   uint64_t C = 0, nnz = 0;

@@ -11,7 +11,7 @@
 //
 // Layout: sliced ELL, slice height 32 (SELL-32).  Rows are ordered for gather locality
 // (classes by first transcript id, transcripts by id) and then bucketed by length inside
-// groups of SELL_GROUP rows, so the 32 rows of a slice have (nearly) equal length.  A
+// groups of rows (SELL_GROUP by default), so the 32 rows of a slice have (nearly) equal length.  A
 // warp owns a slice: lane = row, each lane accumulates its row sequentially in label order.
 // A slice is exactly as wide as its longest row; an entry is a 16-bit index relative to the
 // slice's base index + an 8-byte weight, 10 bytes (run_phase has the column order).  A slice
@@ -39,10 +39,14 @@
 namespace sb {
 namespace cg = cooperative_groups;
 
-constexpr int LMAX_DEFAULT = 96;             // rows longer than this leave the lane-per-row SELL path
-constexpr int LWARP = 2048;                  // ... and are reduced by one warp (<= LWARP) or one block
-constexpr int SELL_GROUP = 1024;             // rows per length-bucketing group
+constexpr uint32_t LMAX = 96;                // rows longer than this leave the lane-per-row SELL path
+constexpr uint32_t LWARP = 2048;             // ... and are reduced by one warp (<= LWARP) or one block
 constexpr int EM_THREADS = 256;
+// Warp ring (WarpRing): EM_CH columns per chunk, EM_RING chunks in flight per warp, EM_MIN_BLOCKS resident blocks per
+// SM (__launch_bounds__).  DESIGN.md 3.4 has the H100 measurements of the other ring shapes.
+constexpr int EM_CH = 8;
+constexpr int EM_RING = 4;
+constexpr int EM_MIN_BLOCKS = 2;
 constexpr double DIGAMMA_MIN = 1e-10;        // CollapsedEMOptimizer.cpp:43
 constexpr double MIN_EQ_W = DBL_MIN;         // :40
 constexpr double ALPHA_CHECK_CUTOFF = 1e-2;  // :884
@@ -158,19 +162,17 @@ __device__ __forceinline__ long long block_sum_ll(long long v, double* scratch) 
 // through a private shared-memory ring with 1-D bulk copies (lane 0 is the producer, the
 // warp is the consumer), so the index/weight stream is never a dependent load and no
 // block-level barrier exists on the data path.
-template <int CH, int RING>   // CH = columns (x32 entries) per chunk, RING = chunks in flight per warp
 struct __align__(128) WarpRing {
-  double w[RING][CH * 32];
-  uint16_t idx[RING][CH * 32];
+  double w[EM_RING][EM_CH * 32];
+  uint16_t idx[EM_RING][EM_CH * 32];
 };
 constexpr int EM_WARPS = EM_THREADS / 32;
-template <int CH, int RING>
-__host__ __device__ constexpr size_t em_smem() { return sizeof(WarpRing<CH, RING>) * EM_WARPS + EM_WARPS * RING * 8 + 40 * 8; }
+// dynamic shared memory of every iteration kernel: the warps' rings, their mbarriers, the block scratch
+constexpr size_t EM_SMEM = sizeof(WarpRing) * EM_WARPS + EM_WARPS * EM_RING * 8 + 40 * 8;
 
-template <int CH, int RING>
 struct WarpCtx {
-  WarpRing<CH, RING>* ring;
-  uint64_t* bars;        // [RING]
+  WarpRing* ring;
+  uint64_t* bars;        // [EM_RING]
   uint32_t phase_bits;   // mbarrier parity per stage
   double* scratch;       // block scratch (40 doubles)
   uint64_t pol_stream;   // L2 eviction policy of the bulk copies (evict_first: the layouts exceed the L2)
@@ -179,12 +181,11 @@ struct WarpCtx {
   unsigned long long t0;
 };
 
-template <int CH, int RING>
-__device__ __forceinline__ void warp_setup(WarpCtx<CH, RING>& W, unsigned char* smem) {
+__device__ __forceinline__ void warp_setup(WarpCtx& W, unsigned char* smem) {
   const uint32_t wid = threadIdx.x >> 5;
-  W.ring = reinterpret_cast<WarpRing<CH, RING>*>(smem) + wid;
-  W.bars = reinterpret_cast<uint64_t*>(smem + sizeof(WarpRing<CH, RING>) * EM_WARPS) + wid * RING;
-  W.scratch = reinterpret_cast<double*>(smem + sizeof(WarpRing<CH, RING>) * EM_WARPS + EM_WARPS * RING * 8);
+  W.ring = reinterpret_cast<WarpRing*>(smem) + wid;
+  W.bars = reinterpret_cast<uint64_t*>(smem + sizeof(WarpRing) * EM_WARPS) + wid * EM_RING;
+  W.scratch = reinterpret_cast<double*>(smem + sizeof(WarpRing) * EM_WARPS + EM_WARPS * EM_RING * 8);
   W.phase_bits = 0;
   W.dbg = nullptr;
   W.dbg_acc = nullptr;
@@ -192,7 +193,7 @@ __device__ __forceinline__ void warp_setup(WarpCtx<CH, RING>& W, unsigned char* 
   W.pol_stream = l2_policy_evict_first();
   if ((threadIdx.x & 31u) == 0) {
 #pragma unroll
-    for (int s = 0; s < RING; ++s) mbar_init(&W.bars[s], 1);
+    for (int s = 0; s < EM_RING; ++s) mbar_init(&W.bars[s], 1);
     mbar_fence_init();
   }
   __syncthreads();
@@ -271,12 +272,11 @@ __device__ __forceinline__ WarpRange load_range(const Sell& S, uint32_t gwarp) {
   r.cend = __ldg(&S.slice_ptr[r.s1]);
   return r;
 }
-template <int CH, int RING>
-__device__ __forceinline__ void ring_issue(const Sell& S, WarpCtx<CH, RING>& W, const WarpRange& R, uint32_t k) {
+__device__ __forceinline__ void ring_issue(const Sell& S, WarpCtx& W, const WarpRange& R, uint32_t k) {
   if ((threadIdx.x & 31u) == 0) {
-    const uint32_t c = R.cbeg + k * CH;
-    const uint32_t cols = min((uint32_t)CH, R.cend - c);
-    const int st = k % RING;
+    const uint32_t c = R.cbeg + k * EM_CH;
+    const uint32_t cols = min((uint32_t)EM_CH, R.cend - c);
+    const int st = k % EM_RING;
     mbar_arrive_expect_tx(&W.bars[st], cols * 320u);
     bulk_g2s_hint(W.ring->w[st], S.w + (size_t)c * 32u, cols * 256u, &W.bars[st], W.pol_stream);
     bulk_g2s_hint(W.ring->idx[st], S.idx + (size_t)c * 32u, cols * 64u, &W.bars[st], W.pol_stream);
@@ -285,19 +285,17 @@ __device__ __forceinline__ void ring_issue(const Sell& S, WarpCtx<CH, RING>& W, 
 // fill the ring with the first chunks of a phase.  The matrices are read-only, so this
 // may run BEFORE the grid barrier that precedes the phase: the stream then lands while
 // the grid synchronises and is never on the critical path.
-template <int CH, int RING>
-__device__ __forceinline__ void ring_prefetch(const Sell& S, WarpCtx<CH, RING>& W, const WarpRange& R) {
-  const uint32_t nchunks = (R.cend - R.cbeg + CH - 1) / CH;
+__device__ __forceinline__ void ring_prefetch(const Sell& S, WarpCtx& W, const WarpRange& R) {
+  const uint32_t nchunks = (R.cend - R.cbeg + EM_CH - 1) / EM_CH;
 #pragma unroll
-  for (int k = 0; k < RING; ++k)
+  for (int k = 0; k < EM_RING; ++k)
     if ((uint32_t)k < nchunks) ring_issue(S, W, R, k);
 }
 // wait for the chunks a speculative ring_prefetch put in flight (before the block retires)
-template <int CH, int RING>
-__device__ __forceinline__ void ring_drain(WarpCtx<CH, RING>& W, const WarpRange& R) {
-  const uint32_t nchunks = (R.cend - R.cbeg + CH - 1) / CH;
+__device__ __forceinline__ void ring_drain(WarpCtx& W, const WarpRange& R) {
+  const uint32_t nchunks = (R.cend - R.cbeg + EM_CH - 1) / EM_CH;
 #pragma unroll
-  for (int k = 0; k < RING; ++k)
+  for (int k = 0; k < EM_RING; ++k)
     if ((uint32_t)k < nchunks) mbar_wait(&W.bars[k], (W.phase_bits >> k) & 1u);
 }
 
@@ -308,26 +306,25 @@ __device__ __forceinline__ void ring_drain(WarpCtx<CH, RING>& W, const WarpRange
 // so a lane reads its four indices with ONE 8-byte load and its four weights with two 16-byte loads and issues the
 // four gathers together; a remainder column is plain column-major (idx[col * 32 + lane]).
 //
-// The range streams through the warp's TMA ring, a circular buffer of CH * RING columns: column c sits at ring column
-// c % (CH * RING), so a group that straddles two chunks is read in place (each lane's four entries are in one chunk: a
-// chunk boundary falls on a multiple of 32 entries) and a chunk is handed back once the stream has passed its last
-// column.
-template <int CH, int RING>
+// The range streams through the warp's TMA ring, a circular buffer of EM_CH * EM_RING columns: column c sits at ring
+// column c % (EM_CH * EM_RING), so a group that straddles two chunks is read in place (each lane's four entries are in
+// one chunk: a chunk boundary falls on a multiple of 32 entries) and a chunk is handed back once the stream has passed
+// its last column.
 struct RingCols {
-  static constexpr uint32_t RC = (uint32_t)(CH * RING);   // ring capacity in columns
+  static constexpr uint32_t RC = (uint32_t)(EM_CH * EM_RING);   // ring capacity in columns
   const Sell& S;
-  WarpCtx<CH, RING>& W;
+  WarpCtx& W;
   const WarpRange& R;
   uint32_t lane, nchunks;
   uint32_t done = 0, ready = 0;             // chunks handed back to the producer / waited for
   // columns [c0, c1) resident: hand back the chunks wholly before c0, wait for those up to column c1 - 1
   __device__ __forceinline__ void need(uint32_t c0, uint32_t c1) {
-    for (; (done + 1u) * CH <= c0; ++done) {
+    for (; (done + 1u) * EM_CH <= c0; ++done) {
       __syncwarp();
-      if (done + RING < nchunks) ring_issue(S, W, R, done + RING);
+      if (done + EM_RING < nchunks) ring_issue(S, W, R, done + EM_RING);
     }
-    for (; ready * CH < c1; ++ready) {
-      const int st = ready % RING;
+    for (; ready * EM_CH < c1; ++ready) {
+      const int st = ready % EM_RING;
       mbar_wait(&W.bars[st], (W.phase_bits >> st) & 1u);
       W.phase_bits ^= (1u << st);
     }
@@ -351,8 +348,8 @@ struct RingCols {
 // remainder columns -- and finished (row_finish) with operands loaded one slice ahead.  The remainder is the same for
 // the 32 lanes, so it is a warp-uniform branch, not a per-lane predicate.  Padding entries (a row shorter than its
 // slice) have weight 0 and gather a slot that always holds 0.0, so a row's sum is its label-order sum.
-template <int PHASE, bool VBEM, int CH, int RING, class Deliver>
-__device__ __forceinline__ void sell_rows(const EmArgs& A, const Sell& S, RingCols<CH, RING>& cols, uint32_t s0,
+template <int PHASE, bool VBEM, class Deliver>
+__device__ __forceinline__ void sell_rows(const EmArgs& A, const Sell& S, RingCols& cols, uint32_t s0,
                                           uint32_t s1, uint32_t cbeg, uint32_t cend, double logNorm, double bias,
                                           P2Acc& pa, Deliver&& deliver) {
   // theta / scale are rewritten by other blocks inside the persistent kernel: plain
@@ -445,17 +442,17 @@ struct Nothing {
 // One phase of a warp: its home range through the ring, then `after_home` (the ring is idle from there on: the caller
 // hands it to the next phase's home range), then the block-path rows, then the phase's work queue: items [0, n_mid)
 // are the warp-path long rows (LMAX < len <= LWARP), longest first, so the short ones fill the end of the phase.
-template <int PHASE, int CH, int RING, bool VBEM, bool DYNQ, class AfterHome, class Deliver>
-__device__ __forceinline__ void run_phase(const EmArgs& A, WarpCtx<CH, RING>& W, const WarpRange& R,
+template <int PHASE, bool VBEM, bool DYNQ, class AfterHome, class Deliver>
+__device__ __forceinline__ void run_phase(const EmArgs& A, WarpCtx& W, const WarpRange& R,
                                           uint32_t bid, uint32_t nblk, double logNorm, double bias,
                                           P2Acc& pa, AfterHome&& after_home, Deliver&& deliver) {
-  static_assert(CH >= 8 && RING >= 2, "two groups in flight span at most two resident chunks");
+  static_assert(EM_CH >= 8 && EM_RING >= 2, "two groups in flight span at most two resident chunks");
   const Sell& S = (PHASE == 1) ? A.cm : A.tm;
   const double* gsrc = (PHASE == 1) ? A.theta : A.scale;
   constexpr bool GUARD = (PHASE == 1) && !VBEM;   // plain EM skips NaN products (:206)
   const uint32_t lane = threadIdx.x & 31u;
   if (R.s1 > R.s0 && R.cend > R.cbeg) {
-    RingCols<CH, RING> rc{S, W, R, lane, (R.cend - R.cbeg + CH - 1) / CH};
+    RingCols rc{S, W, R, lane, (R.cend - R.cbeg + EM_CH - 1) / EM_CH};
     sell_rows<PHASE, VBEM>(A, S, rc, R.s0, R.s1, R.cbeg, R.cend, logNorm, bias, pa, deliver);
     // the chunks still held are not handed back: nothing more to stream in this phase
   }
@@ -647,10 +644,10 @@ __device__ __forceinline__ void p2_finish(const EmArgs& A, double* scratch, P2Ac
   if (dbg_acc && (threadIdx.x & 31u) == 0) A.dbg[(size_t)gwarp * DBG_SLOTS + (slot)] += gtime_ns() - var;
 
 // ---- persistent cooperative kernel: the whole iteration loop, two grid barriers/iter
-template <int CH, int RING, int MINB, bool VBEM>
-__global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent(const __grid_constant__ EmArgs A) {
+template <bool VBEM>
+__global__ void __launch_bounds__(EM_THREADS, EM_MIN_BLOCKS) k_em_persistent(const __grid_constant__ EmArgs A) {
   extern __shared__ __align__(128) unsigned char smem[];
-  WarpCtx<CH, RING> W;
+  WarpCtx W;
   warp_setup(W, smem);
   double* scratch = W.scratch;
   cg::grid_group grid = cg::this_grid();
@@ -672,7 +669,7 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent(const __grid
     SB_ACC_BEGIN(t1, 3)
     W.dbg = (A.dbg && it == A.dbg_it) ? &A.dbg[(size_t)gwarp * DBG_SLOTS] : nullptr;
     // P2's home stream lands while this warp takes queue items and during the grid barrier
-    run_phase<1, CH, RING, VBEM, true>(A, W, R1, bid, nblk, 0.0, 0.0, pa, [&] { ring_prefetch(A.tm, W, R2); }, NoDeliver{});
+    run_phase<1, VBEM, true>(A, W, R1, bid, nblk, 0.0, 0.0, pa, [&] { ring_prefetch(A.tm, W, R2); }, NoDeliver{});
     SB_ACC_END(t1, 0)
     SB_DBG(1)
     grid.sync();
@@ -683,8 +680,7 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent(const __grid
     SB_DBG(3)
     SB_ACC_BEGIN(t2, 4)
     // next iteration's P1 home stream (harmless if the loop ends)
-    run_phase<2, CH, RING, VBEM, true>(A, W, R2, bid, nblk, logNorm, bias, pa, [&] { ring_prefetch(A.cm, W, R1); },
-                                       NoDeliver{});
+    run_phase<2, VBEM, true>(A, W, R2, bid, nblk, logNorm, bias, pa, [&] { ring_prefetch(A.cm, W, R1); }, NoDeliver{});
     W.dbg = nullptr;
     SB_ACC_END(t2, 1)
     SB_DBG(4)
@@ -798,10 +794,10 @@ struct DeliverPush {           // fused path: a flagged line into row `rank` of 
   }
 };
 
-template <int CH, int RING, int MINB, bool VBEM>
-__global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent_mgpu(const __grid_constant__ EmArgs A) {
+template <bool VBEM>
+__global__ void __launch_bounds__(EM_THREADS, EM_MIN_BLOCKS) k_em_persistent_mgpu(const __grid_constant__ EmArgs A) {
   extern __shared__ __align__(128) unsigned char smem[];
-  WarpCtx<CH, RING> W;
+  WarpCtx W;
   warp_setup(W, smem);
   double* scratch = W.scratch;
   cg::grid_group grid = cg::this_grid();
@@ -830,7 +826,7 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent_mgpu(const _
     P2Acc pa{0ll, 0.0};
     SB_DBG(0)
     SB_ACC_BEGIN(t1, 3)
-    run_phase<1, CH, RING, VBEM, true>(A, W, R1, bid, nblk, 0.0, 0.0, pa, [&] { ring_prefetch(A.tm, W, R2); }, NoDeliver{});
+    run_phase<1, VBEM, true>(A, W, R1, bid, nblk, 0.0, 0.0, pa, [&] { ring_prefetch(A.tm, W, R2); }, NoDeliver{});
     SB_ACC_END(t1, 0)
     SB_DBG(1)
     grid.sync();
@@ -840,8 +836,8 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent_mgpu(const _
     if (A.push_pass) {
       // this rank's share of alpha' per transcript id into the local buffer (locally inactive transcripts keep their
       // constant folded singleton mass, written once per run by the host) ...
-      run_phase<3, CH, RING, VBEM, true>(A, W, R2, bid, nblk, 0.0, 0.0, pa, [&] { ring_prefetch(A.cm, W, R1); },
-                                         DeliverLocal{A.part_out});
+      run_phase<3, VBEM, true>(A, W, R2, bid, nblk, 0.0, 0.0, pa, [&] { ring_prefetch(A.cm, W, R1); },
+                               DeliverLocal{A.part_out});
       SB_ACC_END(t2, 1)
       SB_DBG(3)
       __threadfence();
@@ -857,7 +853,7 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent_mgpu(const _
       // straight from the row epilogues; locally inactive transcripts (constant share) first
       for (uint32_t t = gtid; t < M; t += gthreads)
         if (__ldg(&A.tid_row[t]) == 0xffffffffu) push(t, __ldg(&A.base[t]));
-      run_phase<3, CH, RING, VBEM, true>(A, W, R2, bid, nblk, 0.0, 0.0, pa, [&] { ring_prefetch(A.cm, W, R1); }, push);
+      run_phase<3, VBEM, true>(A, W, R2, bid, nblk, 0.0, 0.0, pa, [&] { ring_prefetch(A.cm, W, R1); }, push);
       SB_ACC_END(t2, 1)
       SB_DBG(3)
     }
@@ -970,20 +966,20 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_persistent_mgpu(const _
 }
 
 // ---- one launch per phase (baseline variant; also the NCCL multi-GPU building blocks)
-template <int CH, int RING, int MINB, bool VBEM>
-__global__ void __launch_bounds__(EM_THREADS, MINB) k_em_p1(const __grid_constant__ EmArgs A) {
+template <bool VBEM>
+__global__ void __launch_bounds__(EM_THREADS, EM_MIN_BLOCKS) k_em_p1(const __grid_constant__ EmArgs A) {
   extern __shared__ __align__(128) unsigned char smem[];
-  WarpCtx<CH, RING> W;
+  WarpCtx W;
   warp_setup(W, smem);
   P2Acc pa{0ll, 0.0};
   const WarpRange R = load_range(A.cm, blockIdx.x * (EM_THREADS / 32) + (threadIdx.x >> 5));
   ring_prefetch(A.cm, W, R);
-  run_phase<1, CH, RING, VBEM, false>(A, W, R, blockIdx.x, gridDim.x, 0.0, 0.0, pa, Nothing{}, NoDeliver{});
+  run_phase<1, VBEM, false>(A, W, R, blockIdx.x, gridDim.x, 0.0, 0.0, pa, Nothing{}, NoDeliver{});
 }
-template <int CH, int RING, int MINB, bool VBEM>
-__global__ void __launch_bounds__(EM_THREADS, MINB) k_em_p2(const __grid_constant__ EmArgs A, uint32_t it) {
+template <bool VBEM>
+__global__ void __launch_bounds__(EM_THREADS, EM_MIN_BLOCKS) k_em_p2(const __grid_constant__ EmArgs A, uint32_t it) {
   extern __shared__ __align__(128) unsigned char smem[];
-  WarpCtx<CH, RING> W;
+  WarpCtx W;
   warp_setup(W, smem);
   double* scratch = W.scratch;
   const uint32_t par = it & 1u;
@@ -1001,18 +997,18 @@ __global__ void __launch_bounds__(EM_THREADS, MINB) k_em_p2(const __grid_constan
   P2Acc pa{0ll, 0.0};
   const WarpRange R = load_range(A.tm, blockIdx.x * (EM_THREADS / 32) + (threadIdx.x >> 5));
   ring_prefetch(A.tm, W, R);
-  run_phase<2, CH, RING, VBEM, false>(A, W, R, blockIdx.x, gridDim.x, logNorm, bias, pa, Nothing{}, NoDeliver{});
+  run_phase<2, VBEM, false>(A, W, R, blockIdx.x, gridDim.x, logNorm, bias, pa, Nothing{}, NoDeliver{});
   p2_finish(A, scratch, pa, par);
 }
-template <int CH, int RING, int MINB, bool VBEM>
-__global__ void __launch_bounds__(EM_THREADS, MINB) k_em_p2_partial(const __grid_constant__ EmArgs A) {
+template <bool VBEM>
+__global__ void __launch_bounds__(EM_THREADS, EM_MIN_BLOCKS) k_em_p2_partial(const __grid_constant__ EmArgs A) {
   extern __shared__ __align__(128) unsigned char smem[];
-  WarpCtx<CH, RING> W;
+  WarpCtx W;
   warp_setup(W, smem);
   P2Acc pa{0ll, 0.0};
   const WarpRange R = load_range(A.tm, blockIdx.x * (EM_THREADS / 32) + (threadIdx.x >> 5));
   ring_prefetch(A.tm, W, R);
-  run_phase<3, CH, RING, VBEM, false>(A, W, R, blockIdx.x, gridDim.x, 0.0, 0.0, pa, Nothing{}, DeliverLocal{A.part_out});
+  run_phase<3, VBEM, false>(A, W, R, blockIdx.x, gridDim.x, 0.0, 0.0, pa, Nothing{}, DeliverLocal{A.part_out});
 }
 
 }  // namespace sb

@@ -1,7 +1,7 @@
 """GPU tests of the SELL layout of the EM iteration (H100): exact slice widths (every row length and every
 remainder mod 4, groups of 4 columns straddling ring chunks), 16-bit indices relative to a per-slice base, and the
 long-row fallback of slices whose indices span more than 16 bits -- against the CPU oracle at 1e-9 and bit-identical
-across kernel configurations."""
+across both variants and both ways of cutting the warp ranges."""
 import numpy as np
 import pytest
 
@@ -64,8 +64,8 @@ def local_csr(rng, C, M, lmin, lmax, window=32):
 def test_every_row_length_and_remainder(ctx, oracle, group):
     """Class rows of 2..13 entries, transcript rows of 1..~25.  With groups of 32 rows every slice mixes lengths (one
     slice = one bucketing group); with 1024 the slices are near-uniform, so every width residue mod 4 occurs as a slice
-    of its own.  Every kernel configuration, both ways of cutting the warp ranges and the per-phase kernels give the
-    oracle's alphas, and the same bits.  (At this size a warp's range is about one slice; the ring's wrap-around is
+    of its own.  The persistent and the per-phase kernels, with both ways of cutting the warp ranges, give the oracle's
+    alphas, and the same bits.  (At this size a warp's range is about one slice; the ring's wrap-around is
     test_ranges_wrap_the_ring's.)"""
     rng = np.random.default_rng(11)
     M = 12000
@@ -78,26 +78,26 @@ def test_every_row_length_and_remainder(ctx, oracle, group):
     ctx.set_option("sell_group_cm", group); ctx.set_option("sell_group_tm", group)
     try:
         for rebalance in (0, 3):
-            for cfg, variant in [(0, 1), (1, 1), (2, 1), (3, 1), (1, 0)]:
-                ctx.set_option("config", cfg); ctx.set_option("rebalance", rebalance); ctx.set_option("variant", variant)
+            for variant in (1, 0):
+                ctx.set_option("rebalance", rebalance); ctx.set_option("variant", variant)
                 alpha, st, ok = ctx.optimize(eq, p, proj, eff, uniq)
                 assert ok and st.iters == 12
                 assert ctx.info("fallback_rows_cm") == 0 and ctx.info("fallback_rows_tm") == 0
                 np.testing.assert_allclose(alpha, ref, rtol=ALPHA_RTOL, atol=ALPHA_ATOL)
                 if first is None:
                     first = alpha
-                assert np.array_equal(alpha.view(np.uint64), first.view(np.uint64)), (cfg, variant, rebalance)
+                assert np.array_equal(alpha.view(np.uint64), first.view(np.uint64)), (variant, rebalance)
     finally:
-        ctx.set_option("config", 1); ctx.set_option("rebalance", 1); ctx.set_option("variant", 1)
+        ctx.set_option("rebalance", 1); ctx.set_option("variant", 1)
         ctx.set_option("sell_group_cm", 1024); ctx.set_option("sell_group_tm", 1024)
 
 
 @pytest.mark.parametrize("group", [32, 1024])
 def test_ranges_wrap_the_ring(ctx, oracle, group):
-    """Each warp's range spans several ring lengths, in every kernel configuration, in both layouts: 400 000 classes of
-    2..13 entries and one block per SM (the fewest warps).  So groups of 4 columns start at every offset mod 4 after
-    slices of odd widths and straddle ring chunks, the ring wraps (24 columns with RING = 3, not a power of two; chunks
-    of 16 columns in configuration 0), and chunks are handed back in the middle of slices and between them."""
+    """Each warp's range spans several ring lengths, in both variants, in both layouts: 400 000 classes of 2..13 entries
+    and one block per SM (the fewest warps).  So groups of 4 columns start at every offset mod 4 after slices of odd
+    widths and straddle ring chunks, the ring (4 chunks of 8 columns) wraps, and chunks are handed back in the middle
+    of slices and between them."""
     rng = np.random.default_rng(31)
     M = 200000
     sizes, tids = local_csr(rng, 400000, M, 2, 13)
@@ -109,21 +109,21 @@ def test_ranges_wrap_the_ring(ctx, oracle, group):
     ctx.set_option("sell_group_cm", group); ctx.set_option("sell_group_tm", group)
     try:
         for rebalance in (0, 3):
-            for cfg, variant in [(0, 1), (1, 1), (2, 1), (3, 1), (1, 0)]:
-                ctx.set_option("config", cfg); ctx.set_option("rebalance", rebalance); ctx.set_option("variant", variant)
+            for variant in (1, 0):
+                ctx.set_option("rebalance", rebalance); ctx.set_option("variant", variant)
                 alpha, st, ok = ctx.optimize(eq, p, proj, eff, uniq)
                 assert ok and st.iters == 6
                 assert ctx.info("fallback_rows_cm") == 0 and ctx.info("fallback_rows_tm") == 0
                 warps, ring = ctx.info("warps"), ctx.info("ring_cols")
                 for m in ("cm", "tm"):     # columns per warp: at least two trips around the ring on average
-                    assert ctx.info("sell_cols_" + m) >= 2 * ring * warps, (cfg, m, ctx.info("sell_cols_" + m), warps, ring)
+                    assert ctx.info("sell_cols_" + m) >= 2 * ring * warps, (m, ctx.info("sell_cols_" + m), warps, ring)
                 np.testing.assert_allclose(alpha, ref, rtol=ALPHA_RTOL, atol=ALPHA_ATOL)
                 if first is None:
                     first = alpha
-                assert np.array_equal(alpha.view(np.uint64), first.view(np.uint64)), (cfg, variant, rebalance)
+                assert np.array_equal(alpha.view(np.uint64), first.view(np.uint64)), (variant, rebalance)
     finally:
         ctx.set_option("blocks_per_sm", 0)
-        ctx.set_option("config", 1); ctx.set_option("rebalance", 1); ctx.set_option("variant", 1)
+        ctx.set_option("rebalance", 1); ctx.set_option("variant", 1)
         ctx.set_option("sell_group_cm", 1024); ctx.set_option("sell_group_tm", 1024)
 
 

@@ -270,7 +270,7 @@ typedef struct sb_map_params {
   uint32_t k;                 /* 31 */
   uint32_t stride;            /* seed sampling stride (MAPSPEC) */
   uint32_t max_occs_per_hit;  /* maxOccsPerHit 1000 */
-  uint32_t max_read_occ;      /* maxReadOcc 200 */
+  uint32_t max_read_occ;      /* maxReadOcc 200; at most 1000 (device memory grows with it: DESIGN.md section 14) */
   uint32_t max_frag_len;      /* fragLenDistMax 1000 */
   uint32_t band;              /* bandwidth 15 */
   uint32_t chain_gap;         /* MAPSPEC: diagonal gap inside a chain */
@@ -335,6 +335,13 @@ typedef struct sb_map_params {
 #define SB_LIB_SF 4
 #define SB_LIB_SR 5
 void sb_map_default_params(sb_map_params* p);
+/* salmon's Bowtie2-mimicking presets (rule: DESIGN.md section 14), applied to p after the other options so that they
+ * override them; set lib_type first.  Both: max_read_occ 1000, consensus_frac 0.5 (consensusSlack 0.5), allow_orphans 0
+ * (discardOrphansQuasi) for paired-end library types (a single-end read is a left orphan here and stays), and softclip
+ * mode 1 (--softclipOverhangs) back to 0; mode 2 (--softclip) stays.
+ * strict = 0 (--mimicBT2): ma 2, mp -4, go 5, ge 3.  strict != 0 (--mimicStrictBT2): min_score_fraction 0.8, ma 1,
+ * mp 0, go 25, ge 25.  Returns 0, or SB_ERR_INVALID for a null p. */
+int sb_map_mimic_bt2(sb_map_params* p, int strict);
 
 typedef struct sb_map_batch_stats {
   uint32_t n_pairs;

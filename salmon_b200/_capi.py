@@ -225,6 +225,7 @@ SYMBOLS = {
     "sb_index_info": (C.c_int, [_P, _P]),
     "sb_index_host_arrays": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
     "sb_map_default_params": (None, [C.POINTER(sb_map_params)]),
+    "sb_map_mimic_bt2": (C.c_int, [C.POINTER(sb_map_params), C.c_int]),
     "sb_map_create": (_P, [_P, C.POINTER(sb_map_params), C.c_int, C.c_uint32, C.c_uint32]),
     "sb_map_destroy": (None, [_P]),
     "sb_map_batch": (C.c_int, [_P, _P, _P, C.c_uint32, C.c_uint32, C.POINTER(sb_map_batch_stats)]),
@@ -561,6 +562,13 @@ def map_default_params(**over) -> sb_map_params:
         if not hasattr(p, k):
             raise AttributeError(k)
         setattr(p, k, v)
+    return p
+
+
+def map_mimic_bt2(p: sb_map_params, strict=False) -> sb_map_params:
+    """sb_map_mimic_bt2: salmon's `--mimicBT2` (strict False) or `--mimicStrictBT2` (strict True) presets applied to p in
+    place, overriding the values p holds for the same options (DESIGN.md section 14).  Returns p."""
+    _check(load().sb_map_mimic_bt2(C.byref(p), 1 if strict else 0), "sb_map_mimic_bt2")
     return p
 
 

@@ -76,6 +76,7 @@ int usage() {
           "  sb_salmon quant -i index_dir -l IU|ISF|ISR -1 r1.fq[.gz] ... -2 r2.fq[.gz] ... | -l U|SF|SR -r reads.fq[.gz] ...  -o out_dir [--gpus N]\n"
           "                  [-p threads] [--dumpEq] [--dumpEqWeights] [--writeMappings[=FILE] | -z] [--writeQualities] [--writeUnmappedNames]\n"
           "                  [--recoverOrphans] [--softclip] [--softclipOverhangs] [--incompatPrior 0] [--noSingleFragProb]\n"
+          "                  [--mimicBT2 | --mimicStrictBT2] [--minAlnProb 1e-5]\n"
           "                  [--noFragLengthDist --noEffectiveLengthCorrection | --noEffectiveLengthCorrection]\n"
           "                  [--numBootstraps N | --numGibbsSamples N] [--thinningFactor 16] [--noGammaDraw] [--useEM] [--vbPrior 0.01]\n"
           "                  [--perNucleotidePrior] [--maxReadOcc 200] [--maxOccsPerHit 1000] [--minScoreFraction 0.65] [--consensusSlack 0.35]\n"
@@ -213,7 +214,7 @@ int cmd_quant(Args& a) {
   sb_quant_default_opts(&qo);
   auto num = [&](double& d) { if (!a.value(v)) return false; d = atof(v.c_str()); return true; };
   double d = 0;
-  bool vb_prior_given = false, pre_merge_given = false, threads_given = false;
+  bool vb_prior_given = false, pre_merge_given = false, threads_given = false, mimic = false, mimic_strict = false;
   int n_gpus = 1, my_rank = -1;
   std::string run_tag, sam_path;
   while (a.more()) {
@@ -289,6 +290,18 @@ int cmd_quant(Args& a) {
       // 0 or below 1e-100: incompatible mappings are ignored (QuantOptionsUtils.cpp:608-616)
       mp.incompat_prior = (x == 0.0 || x < 1e-100) ? 0.0 : x;
     }
+    else if (o == "--minAlnProb") {
+      if (!a.value(v)) return usage();
+      char* end = nullptr;
+      const double x = strtod(v.c_str(), &end);
+      if (v.empty() || *end != '\0' || !(x >= 0.0 && x <= 1.0)) {
+        fprintf(stderr, "sb_salmon quant: --minAlnProb takes a probability in [0, 1], got '%s'\n", v.c_str());
+        return 1;
+      }
+      mp.min_aln_prob = x;
+    }
+    else if (o == "--mimicBT2") mimic = true;
+    else if (o == "--mimicStrictBT2") mimic_strict = true;
     else if (o == "--noSingleFragProb") mp.no_single_frag_prob = 1;
     else if (o == "--noFragLengthDist") mp.no_frag_len_dist = 1;
     else if (o == "--noEffectiveLengthCorrection") mp.no_eff_len_correction = 1;
@@ -299,6 +312,11 @@ int cmd_quant(Args& a) {
     } else { fprintf(stderr, "sb_salmon quant: unknown option %s\n", o.c_str()); return usage(); }
   }
   if (out.empty()) return usage();
+  if (mimic && mimic_strict) {   // QuantOptionsUtils.cpp:250-254
+    fprintf(stderr, "sb_salmon quant: You passed both the --mimicBT2 and --mimicStrictBT2 parameters.  These are mutually "
+                    "exclusive. Please select only one of these flags.\n");
+    return 1;
+  }
   if (mp.no_frag_len_dist && !mp.no_eff_len_correction) {   // QuantOptionsUtils.cpp:641-647
     fprintf(stderr, "sb_salmon quant: You cannot enable --noFragLengthDist without also enabling --noEffectiveLengthCorrection\n");
     return 1;
@@ -399,6 +417,21 @@ int cmd_quant(Args& a) {
     return 1;
   }
   mp.lib_type = lib_id;
+  if (mimic || mimic_strict) {   // the presets override the values given for the same options (:256-289)
+    const bool overhangs = mp.softclip == 1;
+    sb_map_mimic_bt2(&mp, mimic_strict ? 1 : 0);
+    if (my_rank <= 0) {
+      fprintf(stderr, "[info] The --mimicBT2 and --mimicStrictBT2 flags increases maxReadOccs to %u.\n", mp.max_read_occ);
+      fprintf(stderr, "[info] The --mimicBT2 and --mimicStrictBT2 flags increases consensusSlack to %g.\n", 1.0 - mp.consensus_frac);
+      fprintf(stderr, mimic_strict ? "[info] Usage of --mimicStrictBT2 overrides other settings for mapping validation. Setting "
+                                     "strict RSEM+Bowtie2-like parameters now.\n"
+                                   : "[info] Usage of --mimicBT2 overrides other settings for mapping validation. Setting "
+                                     "Bowtie2-like parameters now.\n");
+      if (overhangs)
+        fprintf(stderr, "[info] Softclipping of overhangs is not allowed in %s mode; setting to false.\n",
+                mimic_strict ? "mimicStrictBT2" : "mimicBT2");
+    }
+  }
   if (se_input && !pre_merge_given) mp.pre_merge_thresh = 1.0;    // single-end default (QuantOptionsUtils.cpp:215-218)
   if (se_input) mp.recover_orphans = 0;   // a single-end read has no mate to rescue: accepted, no effect (as in salmon)
   // the CUDA context comes up (seconds) while the index is read from disk

@@ -1071,11 +1071,24 @@ static inline unsigned nblk(uint64_t n, unsigned t) { return (unsigned)((n + t -
 // other scores set_option("fast_dp", 1) leaves it off
 static inline int fast_dp_exact(const Params& p) { return (p.ma >= 0 && p.mp <= p.ma && p.go >= 0 && p.ge >= 0) ? 1 : 0; }
 
+// gapless settlement of k_dp_classify (DESIGN.md section 14): in scoring mode 0, when every gapped path scores below the
+// lowest mate score that can change an outcome, the best ungapped diagonal settles every alignment.  The thresholds are
+// evaluated exactly as assign_read and rescue_mate_passes evaluate them, at the highest score a gapped path can reach
+// (G = ma*L - go - ge) and, for a pair, with a perfect partner.  Decided per launch: it depends on L.
+static inline int gapless_settles(const Params& p, uint32_t L) {
+  if (p.softclip != 0) return 0;
+  const int32_t perfect = p.ma * (int32_t)L, G = perfect - p.go - p.ge;
+  if (!((double)G < p.min_score_fraction * (double)perfect)) return 0;   // orphans, single-end reads, rescue
+  if (p.lib_type < 3 && !((double)(G + perfect) < p.min_score_fraction * (double)(2 * perfect))) return 0;   // pairs
+  return 1;
+}
+
 // the three DP kernels of one chunk for scoring mode MODE (Params::softclip); the same launches in every mode
 template <int NWR, int MODE>
 static void launch_dp(const sb_map_ctx* c, cudaStream_t st, const IndexView& ix, const Params& p, uint32_t L,
                       const uint8_t* dl, const uint8_t* dr, const DpIo& io) {
-  k_dp_classify<NWR, MODE><<<c->n_sm * 3, 256, 0, st>>>(ix, p, c->pr, L, c->fast_ok, io);
+  const int gapless = (c->fast_ok && gapless_settles(p, L)) ? 1 : 0;
+  k_dp_classify<NWR, MODE><<<c->n_sm * 3, 256, 0, st>>>(ix, p, c->pr, L, c->fast_ok, gapless, io);
   k_dp_pair<NWR, MODE == 2 ? 2 : 0><<<c->n_sm * (NWR == 4 ? 3 : 2), 256, 0, st>>>(ix, p, c->pr, L, io);
   k_dp_general<NWR, MODE><<<c->n_sm * 3, 256, 0, st>>>(ix, p, c->pr, dl, dr, L, c->ascii, io);
 }
@@ -1090,6 +1103,20 @@ extern "C" void sb_map_default_params(sb_map_params* q) {
   q->seed = 42; q->mini_batch = 5000;
   q->pre_merge_thresh = 0.75; q->post_merge_thresh = 0.9; q->orphan_thresh = 0.95;   // SalmonDefaults.hpp:28-30
   q->allow_dovetail = 0; q->allow_orphans = 1;                                         // :46, discardOrphansQuasi = false
+}
+
+// --mimicBT2 / --mimicStrictBT2 (QuantOptionsUtils.cpp:250-289), applied after the other options so that it overrides them
+extern "C" int sb_map_mimic_bt2(sb_map_params* q, int strict) {
+  if (!q) { sb::set_error("null argument"); return SB_ERR_INVALID; }
+  q->max_read_occ = 1000;
+  q->consensus_frac = 1.0 - 0.5;        // consensusSlack 0.5
+  // discardOrphansQuasi concerns the mates of pairs: a single-end read is a left orphan in this mapper, so it stays
+  const bool single_end = (q->lib_type >= SB_LIB_U && q->lib_type <= SB_LIB_SR) || q->lib_type == SB_LIB_AUTO_SINGLE;
+  if (!single_end) q->allow_orphans = 0;
+  if (q->softclip == 1) q->softclip = 0;   // softclipOverhangs off; --softclip (mode 2) stays
+  if (strict) { q->min_score_fraction = 0.8; q->ma = 1; q->mp = 0; q->go = 25; q->ge = 25; }
+  else { q->ma = 2; q->mp = -4; q->go = 5; q->ge = 3; }
+  return SB_OK;
 }
 
 static void build_fld_host(const Params& p, std::vector<double>& t) {
@@ -1175,6 +1202,10 @@ extern "C" sb_map_ctx* sb_map_create(sb_index* ix, const sb_map_params* q, int d
     sb::set_error("sb_map_create: incompat_prior must be a probability in [0, 1], got %g", q->incompat_prior);
     return nullptr;
   }
+  if (q->max_read_occ > MAX_READ_OCC) {
+    sb::set_error("sb_map_create: max_read_occ %u is above the supported %u (--maxReadOcc)", q->max_read_occ, MAX_READ_OCC);
+    return nullptr;
+  }
   if (q->no_frag_len_dist && !q->no_eff_len_correction) {   // QuantOptionsUtils.cpp:641-647
     sb::set_error("sb_map_create: no_frag_len_dist needs no_eff_len_correction (--noFragLengthDist without "
                   "--noEffectiveLengthCorrection)");
@@ -1186,10 +1217,10 @@ extern "C" sb_map_ctx* sb_map_create(sb_index* ix, const sb_map_params* q, int d
     sb::set_error("no CUDA device available (libsalmon_b200 has no CPU fallback)");
     return nullptr;
   }
-  if (q->band > 15 || q->max_read_occ > 255 || max_read_len > 256 || q->k != ix->k || batch_cap == 0 ||
+  if (q->band > 15 || max_read_len > 256 || q->k != ix->k || batch_cap == 0 ||
       batch_cap > (1u << 24) || q->stride == 0 || max_read_len < q->k ||
       (max_read_len - q->k) / q->stride + 2 > MAX_LOOKUPS) {
-    sb::set_error("sb_map_create: unsupported parameters (band<=15, max_read_occ<=255, read_len<=256, k must match "
+    sb::set_error("sb_map_create: unsupported parameters (band<=15, read_len<=256, k must match "
                   "the index, at most %u seed positions per mate)", MAX_LOOKUPS);
     return nullptr;
   }

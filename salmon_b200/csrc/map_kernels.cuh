@@ -24,6 +24,7 @@ namespace sbmap {
 constexpr int SEED_WARPS = 8;        // warps per block of k_seed_chain_w
 constexpr int SK = 512;              // seed keys per warp held in shared memory (more: global scratch)
 constexpr uint32_t MAX_LOOKUPS = 64; // seed positions per mate handled by the warp kernel (2 rounds of 32)
+constexpr uint32_t MAX_READ_OCC = 1000;   // largest max_read_occ (--maxReadOcc; the value --mimicBT2 sets)
 
 struct PackedReads {
   uint64_t* bits;    // [(2*n) * wpr]  base j of a mate at bits 2*(j&31) of word j>>5 (N stored as 0)
@@ -760,9 +761,23 @@ __device__ __forceinline__ void load_window(const IndexView& ix, int64_t tbase, 
 //   mode 2: only interior alignments, and only a perfect diagonal settles the alignment: ma*L is the most any path can
 //           score, while a full-length diagonal with a mismatch may be beaten by a clipped run of the same diagonal, so
 //           the DP scores those.
+//
+// Gapless settlement (gapless = 1, decided per launch by the host, mode 0 only; DESIGN.md section 14): the best
+// ungapped score u settles the alignment whatever it is, when G = ma*L - go - ge < s_min, where s_min is the lowest mate
+// score that can still change an outcome.  A hit's score is the sum of its mates' scores and passes when it reaches
+// minScoreFraction * ma * L per mate; no mate scores above ma*L.  So a mate of a passing pair scores at least
+// s_min = (2*minScoreFraction - 1)*ma*L (its partner perfect), and a passing orphan, single-end read, rescue anchor or
+// rescued mate at least minScoreFraction*ma*L >= s_min.  Let d = max(u, best gapped score) be the DP's score; the best
+// gapped score is at most G.
+//   - d >= s_min: then d > G, so d = u.
+//   - d < s_min: then u <= d < s_min too, and every hit with this mate fails its threshold with either value (or is
+//     invalid: u = NEG_SCORE when no diagonal fits inside the transcript), so it is INVALID_SCORE either way.
+// Hit scores, hence the decoy maximum, the filters and the written alignments, are the same; the rescue anchors pass
+// rescue_mate_passes with u exactly when with d; the per-mate scores SAM writes belong to passing hits, where u = d.
+// The host compares in double exactly as assign_read and rescue_mate_passes do, at G (single mate) and G + ma*L (pair).
 template <int NWR, int MODE>   // read words: 4 (read_len <= 128) or 8 (<= 256)
 __global__ void __launch_bounds__(256, 3)
-k_dp_classify(IndexView ix, Params p, PackedReads pr, uint32_t L, int fast_ok, DpIo io) {
+k_dp_classify(IndexView ix, Params p, PackedReads pr, uint32_t L, int fast_ok, int gapless, DpIo io) {
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t ntasks = *io.n_tasks;
   const uint32_t nthreads = gridDim.x * blockDim.x;
@@ -813,7 +828,7 @@ k_dp_classify(IndexView ix, Params p, PackedReads pr, uint32_t L, int fast_ok, D
             if (best_u == perfect) break;
           }
         }
-        if (try_fast && best_u >= (MODE == 2 ? perfect : bound)) {
+        if (try_fast && (gapless || best_u >= (MODE == 2 ? perfect : bound))) {
           (mate ? io.score_r : io.score_l)[(size_t)r * MAXCAND + ci] = best_u;
         } else {
           dest = interior ? 0 : 1;

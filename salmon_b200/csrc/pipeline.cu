@@ -438,14 +438,19 @@ int write_run_metadata(const std::string& outs, const MetaIn& m) {
              "    \"num_processed\": %llu,\n    \"num_mapped\": %llu,\n    \"num_decoy_fragments\": 0,\n    \"num_dovetail_fragments\": 0,\n"
              "    \"num_fragments_filtered_vm\": 0,\n    \"num_alignments_below_threshold_for_mapped_fragments_vm\": 0,\n"
              "    \"percent_mapped\": %.6f,\n    \"call\": \"quant\",\n    \"start_time\": \"%s\",\n    \"end_time\": \"%s\",\n    \"sb_num_gpus\": %d,\n"
-             "    \"sb_num_orphans_rescued\": %llu\n}\n",
+             "    \"sb_num_orphans_rescued\": %llu,\n"
+             "    \"sb_mapping_params\": {\"max_read_occ\": %u, \"consensus_slack\": %.15g, \"min_score_fraction\": %.15g, "
+             "\"min_aln_prob\": %.15g, \"ma\": %d, \"mp\": %d, \"go\": %d, \"ge\": %d, \"discard_orphans\": %s, "
+             "\"softclip\": %s, \"softclip_overhangs\": %s}\n}\n",
              sb_version(), m.o->num_bootstraps ? "bootstrap" : (m.o->num_gibbs ? "gibbs" : "none"), m.ep->use_vbem ? "vb" : "em",
              (m.mp->lib_type >= 0 && m.mp->lib_type <= 5) ? (const char* const[]){"IU", "ISF", "ISR", "U", "SF", "SR"}[m.mp->lib_type] : "IU",
              pmf.size(), mean, sd, m.n_valid, m.n_decoy, (unsigned long long)m.n_classes,
              (m.o->dump_eq || m.o->dump_eq_weights) ? "true" : "false",
              m.mp->range_bins ? "\n        \"range_factorized\"\n    " : "", n_samp, (unsigned long long)m.n_observed,
              (unsigned long long)m.n_mapped, pct, m.start_time.c_str(), m.end_time.c_str(), m.n_ranks,
-             (unsigned long long)m.orphans_rescued);
+             (unsigned long long)m.orphans_rescued, m.mp->max_read_occ, 1.0 - m.mp->consensus_frac, m.mp->min_score_fraction,
+             m.mp->min_aln_prob, m.mp->ma, m.mp->mp, m.mp->go, m.mp->ge, m.mp->allow_orphans ? "false" : "true",
+             m.mp->softclip == 2 ? "true" : "false", m.mp->softclip >= 1 ? "true" : "false");
     ok = write_text(outs + "/aux_info/meta_info.json", buf) && ok;
   }
   {   // lib_format_counts.json (ReadExperiment.inl:219-350): compatible = assigned fragments with at least one kept mapping

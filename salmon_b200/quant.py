@@ -41,6 +41,21 @@ def _likelihood_options(mp, incompat_prior, no_single_frag_prob, no_frag_len_dis
     return mp
 
 
+def _mimic_options(mp, min_aln_prob, mimic_bt2, mimic_strict_bt2):
+    """`--minAlnProb`, then `--mimicBT2` / `--mimicStrictBT2` (sb_map_mimic_bt2, DESIGN.md section 14), which override
+    the values given for the same options; the defaults leave mp as it is"""
+    if mimic_bt2 and mimic_strict_bt2:
+        raise _capi.SalmonB200Error("You passed both the --mimicBT2 and --mimicStrictBT2 parameters.  These are mutually "
+                                    "exclusive. Please select only one of these flags.")
+    if min_aln_prob is not None:
+        if not 0.0 <= float(min_aln_prob) <= 1.0:
+            raise _capi.SalmonB200Error(f"--minAlnProb takes a probability in [0, 1], got {min_aln_prob}")
+        mp.min_aln_prob = float(min_aln_prob)
+    if mimic_bt2 or mimic_strict_bt2:
+        _capi.map_mimic_bt2(mp, strict=bool(mimic_strict_bt2))
+    return mp
+
+
 def _drop_decoys(index, inputs):
     """readExp.dropDecoyTranscripts() (SalmonQuantify.cpp:2479, ReadExperiment.hpp:120): decoys -- the suffix of the id
     space, never part of a label -- leave before the optimiser and the writers.  Returns (Mq, inputs cut to Mq)."""
@@ -58,13 +73,16 @@ def _drop_decoys(index, inputs):
 
 def quant_reads(index, left, right, map_params=None, em_params=None, device=0, batch=262_144, dist=None,
                 names=None, out_dir=None, dump_eq=False, dump_eq_weights=False, incompat_prior=0.0,
-                no_single_frag_prob=False, no_frag_len_dist=False, no_eff_len_correction=False):
+                no_single_frag_prob=False, no_frag_len_dist=False, no_eff_len_correction=False, min_aln_prob=None,
+                mimic_bt2=False, mimic_strict_bt2=False):
     """left/right: [n, L] uint8 base codes (0..3 = ACGT, 4 = N) of THIS rank's read shard.  incompat_prior,
     no_single_frag_prob, no_frag_len_dist, no_eff_len_correction: `--incompatPrior`, `--noSingleFragProb`,
-    `--noFragLengthDist`, `--noEffectiveLengthCorrection` (set on map_params; DESIGN.md section 13).
+    `--noFragLengthDist`, `--noEffectiveLengthCorrection` (set on map_params; DESIGN.md section 13).  min_aln_prob,
+    mimic_bt2, mimic_strict_bt2: `--minAlnProb`, `--mimicBT2`, `--mimicStrictBT2` (DESIGN.md section 14).
     Returns dict(alpha, tpm, eff_len, classes, n_mapped, em_stats)."""
     mp = _likelihood_options(map_params or map_default_params(), incompat_prior, no_single_frag_prob, no_frag_len_dist,
                              no_eff_len_correction)
+    _mimic_options(mp, min_aln_prob, mimic_bt2, mimic_strict_bt2)
     ep = em_params or default_params()
     n, L = left.shape
     world = dist.get_world_size() if (dist is not None and dist.is_initialized()) else 1
@@ -162,7 +180,7 @@ def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=
                 max_read_len=256, threads=8, dist=None, dump_eq=False, dump_eq_weights=False, num_bootstraps=0, seed=0,
                 write_mappings=None, write_qualities=False, write_unmapped_names=False, cmdline="", recover_orphans=False,
                 softclip=0, incompat_prior=0.0, no_single_frag_prob=False, no_frag_len_dist=False,
-                no_eff_len_correction=False):
+                no_eff_len_correction=False, min_aln_prob=None, mimic_bt2=False, mimic_strict_bt2=False):
     """`salmon quant -i index -l IU -1 mates1 -2 mates2 -o out_dir` for the hot path: FASTQ/FASTA(.gz) files ->
     sb_reads_bucketed -> sb_map_batch -> ... -> quant.sf.  index: an _capi.Index or the path of a saved one.  With
     torch.distributed initialised every rank takes the global batches g with g % world == rank (round-robin sharding
@@ -174,7 +192,8 @@ def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=
     softclip: scoring mode of the DP (sets map_params.softclip when non-zero): 1 = `--softclipOverhangs`, 2 =
     `--softclip` (DESIGN.md section 12).  incompat_prior, no_single_frag_prob, no_frag_len_dist, no_eff_len_correction:
     `--incompatPrior`, `--noSingleFragProb`, `--noFragLengthDist`, `--noEffectiveLengthCorrection` (DESIGN.md section
-    13)."""
+    13).  min_aln_prob, mimic_bt2, mimic_strict_bt2: `--minAlnProb`, `--mimicBT2`, `--mimicStrictBT2`, applied after the
+    other options so that the presets override them (DESIGN.md section 14)."""
     if isinstance(index, (str, bytes, os.PathLike)):
         index = _capi.Index.load(index)
     mp = map_params or map_default_params()
@@ -183,6 +202,7 @@ def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=
     if softclip:
         mp.softclip = int(softclip)
     _likelihood_options(mp, incompat_prior, no_single_frag_prob, no_frag_len_dist, no_eff_len_correction)
+    _mimic_options(mp, min_aln_prob, mimic_bt2, mimic_strict_bt2)
     meta = index.meta()
     if meta["first_decoy"] < index.n_txps:
         mp.first_decoy = meta["first_decoy"]

@@ -468,6 +468,10 @@ int sb_rescue_search_tap(int device, uint32_t n, const uint8_t* pats, const uint
 int sb_map_last_alignments(sb_map_ctx* ctx, uint32_t n, uint32_t* n_aln, uint32_t* tid, int32_t* score,
                            double* prob, int32_t* pos, int32_t* mate_pos, uint8_t* flags, int32_t* flen,
                            uint32_t* label, double* weight);
+/* Parity tap: the per-read candidates of the last batch as the seed kernel left them: n_l / n_r [n] (bit 31 of n_l set:
+ * the read has no joint hit or more than max_read_occ of them), cand_l / cand_r [n * 64] of 12 bytes each (tid, diag_c,
+ * orientation << 31 | coverage).  SB_ERR_STATE when the last batch ran as more than one chunk or with orphan rescue. */
+int sb_map_last_candidates(sb_map_ctx* ctx, uint32_t n, uint32_t* n_l, uint32_t* n_r, void* cand_l, void* cand_r);
 
 /* The read stream as [n, L] batches of one read length each (what sb_map_batch takes): a reader thread parses, groups
  * the reads by length into double-buffered (page-locked, when a device is present) matrices and hands full ones to

@@ -213,14 +213,16 @@ static int cmp_cand_pos(const void* a, const void* b) {
   return x->diag_c < y->diag_c ? -1 : (x->diag_c > y->diag_c);
 }
 
-static uint32_t mate_candidates(const orc_index* ix, const orc_map_params* p, const uint8_t* read,
-                                uint32_t L, cand_t* out, orc_map_counters* ctr) {
+/* info (may be NULL): what the mate's seeds look like, see orc_mate_candidates */
+static uint32_t mate_candidates_info(const orc_index* ix, const orc_map_params* p, const uint8_t* read,
+                                     uint32_t L, cand_t* out, orc_map_counters* ctr, orc_mate_info* info) {
   const uint32_t K = p->k;
+  if (info) memset(info, 0, sizeof(*info));
   if (L < K) return 0;
   seed_t* seeds = (seed_t*)malloc(MAXSEEDS * sizeof(seed_t));
   uint32_t ns = 0;
   /* sample positions 0, S, 2S, ... and the last k-mer */
-  for (uint32_t i = 0;; i += p->stride) {
+  for (uint32_t i = 0, pi = 0;; i += p->stride, ++pi) {
     uint32_t pos_i = i;
     int last = 0;
     if (i > L - K) { if ((L - K) % p->stride == 0) break; pos_i = L - K; last = 1; }
@@ -234,6 +236,10 @@ static uint32_t mate_candidates(const orc_index* ix, const orc_map_params* p, co
       if (h >= 0) {
         uint64_t b = ix->post_off[h], e = ix->post_off[h + 1];
         if (e - b <= p->max_occs_per_hit) {
+          if (info) {
+            if (!info->cut_round && ns + (e - b) > MAXSEEDS) info->cut_round = 1 + pi / 32;
+            info->postings_all += (uint32_t)(e - b);
+          }
           for (uint64_t q = b; q < e && ns < MAXSEEDS; ++q) {
             ctr->postings++;
             uint64_t gp = ix->post[q];
@@ -253,6 +259,10 @@ static uint32_t mate_candidates(const orc_index* ix, const orc_map_params* p, co
     }
     if (last) break;
   }
+  if (info) {
+    info->lookups = (uint32_t)ctr->lookups;   /* the caller passes fresh counters */
+    info->seeds = ns;
+  }
   ctr->seeds += ns;
   qsort(seeds, ns, sizeof(seed_t), cmp_seed);
   /* chains: same (tid, ori), consecutive diagonals at most chain_gap apart */
@@ -269,6 +279,14 @@ static uint32_t mate_candidates(const orc_index* ix, const orc_map_params* p, co
       for (uint32_t b = 0; b < K; ++b) { int32_t q = seeds[s].qpos + (int32_t)b; if (q >= 0 && q < 256) covered[q] = 1; }
     uint32_t cov = 0;
     for (uint32_t b = 0; b < 256; ++b) cov += covered[b];
+    if (info) {   /* the chain spans seeds i..j-1: does it cross a 32-key chunk of the seed array / of the array of
+                   * distinct (tid, ori, diag) keys? */
+      uint32_t d0 = info->distinct;
+      for (uint32_t s = i; s < j; ++s)
+        if (s == i || seeds[s].diag != seeds[s - 1].diag) ++info->distinct;
+      info->straddle_seeds += (i / 32 != (j - 1) / 32);
+      info->straddle_distinct += (d0 / 32 != (info->distinct - 1) / 32);
+    }
     cand_t c;
     c.tid = seeds[i].tid; c.ori = seeds[i].ori; c.dmin = seeds[i].diag; c.dmax = seeds[j - 1].diag;
     c.diag_c = c.dmin + (c.dmax - c.dmin) / 2; c.cov = cov;
@@ -280,11 +298,30 @@ static uint32_t mate_candidates(const orc_index* ix, const orc_map_params* p, co
   uint32_t nk = 0;
   for (uint32_t c = 0; c < nc; ++c)
     if ((double)all[c].cov >= p->consensus_frac * (double)best) all[nk++] = all[c];
+  if (info) { info->chains = nc; info->survivors = nk; }
   if (nk > MAXCAND) { qsort(all, nk, sizeof(cand_t), cmp_cand_cov); nk = MAXCAND; }
   qsort(all, nk, sizeof(cand_t), cmp_cand_pos);
   memcpy(out, all, nk * sizeof(cand_t));
   free(all); free(seeds);
   return nk;
+}
+
+static uint32_t mate_candidates(const orc_index* ix, const orc_map_params* p, const uint8_t* read,
+                                uint32_t L, cand_t* out, orc_map_counters* ctr) {
+  return mate_candidates_info(ix, p, read, L, out, ctr, NULL);
+}
+
+/* test hook: the candidates of one mate in (tid, ori, diag_c) order, as orc_map_reads derives them */
+uint32_t orc_mate_candidates(const orc_index* ix, const orc_map_params* p, const uint8_t* read, uint32_t L,
+                             orc_cand* out, orc_mate_info* info) {
+  cand_t c[MAXCAND];
+  orc_map_counters ctr;
+  memset(&ctr, 0, sizeof ctr);
+  const uint32_t n = mate_candidates_info(ix, p, read, L, c, &ctr, info);
+  for (uint32_t a = 0; a < n; ++a) {
+    out[a].tid = c[a].tid; out[a].ori = c[a].ori; out[a].diag_c = c[a].diag_c; out[a].cov = c[a].cov;
+  }
+  return n;
 }
 
 /* ---------------------------------------------------------------- banded affine glocal DP */

@@ -126,6 +126,23 @@ void orc_math_probe(int mode, uint64_t nx, const double* x, double* ex, uint64_t
 int32_t orc_dp_score(const orc_index* ix, const orc_map_params* p, const uint8_t* read, uint32_t L, uint32_t ori,
                      uint32_t tid, int32_t diag_c);
 
+/* test hook: the candidates of one mate (at most 64, in (tid, ori, diag_c) order) and what its seeds look like.  The
+ * fields tell which path of the product's seed kernel the mate takes (tests/test_seed_paths_cpu.py). */
+typedef struct orc_cand { uint32_t tid, ori; int32_t diag_c; uint32_t cov; } orc_cand;
+typedef struct orc_mate_info {
+  uint32_t lookups;            /* valid k-mer lookups (no N) */
+  uint32_t postings_all;       /* postings of the accepted lookups, before the 2048-seed cut */
+  uint32_t seeds;              /* seeds kept (after the cut) */
+  uint32_t cut_round;          /* 0: no cut; else the round of 32 seed positions whose lookup the cut fell in (1, 2) */
+  uint32_t distinct;           /* distinct (tid, ori, diag) keys among the kept seeds */
+  uint32_t chains;
+  uint32_t survivors;          /* chains at or above the consensus threshold, before the top-64 cut */
+  uint32_t straddle_seeds;     /* chains whose seeds cross a 32-key boundary of the sorted seed array */
+  uint32_t straddle_distinct;  /* the same over the sorted array of distinct keys */
+} orc_mate_info;
+uint32_t orc_mate_candidates(const orc_index* ix, const orc_map_params* p, const uint8_t* read, uint32_t L,
+                             orc_cand* out /*[64]*/, orc_mate_info* info);
+
 #ifdef __cplusplus
 }
 #endif

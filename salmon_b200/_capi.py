@@ -253,6 +253,7 @@ SYMBOLS = {
     "sb_map_partial_get": (C.c_int, [_P, C.POINTER(sb_map_partial)]),
     "sb_map_project_global": (C.c_int, [_P, C.POINTER(sb_map_partial), C.c_uint32, _P, C.POINTER(sb_map_result)]),
     "sb_map_last_alignments": (C.c_int, [_P, C.c_uint32] + [_P] * 10),
+    "sb_map_last_candidates": (C.c_int, [_P, C.c_uint32] + [_P] * 4),
     "sb_rescue_search_tap": (C.c_int, [C.c_int, C.c_uint32] + [_P] * 7),
     "sb_sam_open": (_P, [C.c_char_p, C.c_char_p, _P, C.c_char_p, C.c_uint32]),
     "sb_sam_close": (C.c_int, [_P]),
@@ -660,6 +661,9 @@ class Index:
             pass
 
 
+CAND_DTYPE = np.dtype([("tid", np.uint32), ("diag_c", np.int32), ("ori_cov", np.uint32)])   # sbmap::Cand
+
+
 def alloc_alignment_arrays(n, cap):
     return dict(n_aln=np.zeros(n, dtype=np.uint32), tid=np.zeros((n, cap), dtype=np.uint32),
                 score=np.zeros((n, cap), dtype=np.int32), prob=np.zeros((n, cap)),
@@ -773,6 +777,16 @@ class MapContext:
             "n_aln", "tid", "score", "prob", "pos", "mate_pos", "flags", "flen", "label", "weight")]),
             "sb_map_last_alignments")
         return a
+
+    def last_candidates(self):
+        """the seed kernel's candidates of the last batch: n_l, n_r [n] (bit 31 of n_l: unmapped) and cand_l, cand_r
+        [n, 64] records (tid, diag_c, ori_cov); refused after a batch of several chunks or with orphan rescue"""
+        n = self.last_n
+        out = dict(n_l=np.zeros(n, np.uint32), n_r=np.zeros(n, np.uint32), cand_l=np.zeros((n, 64), CAND_DTYPE),
+                   cand_r=np.zeros((n, 64), CAND_DTYPE))
+        _check(self.lib.sb_map_last_candidates(self.h, n, *[out[k].ctypes.data for k in ("n_l", "n_r", "cand_l", "cand_r")]),
+               "sb_map_last_candidates")
+        return out
 
     def finish(self):
         r = sb_map_result()

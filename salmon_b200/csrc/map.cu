@@ -1042,6 +1042,8 @@ struct sb_map_ctx {
   uint64_t full_dp_total = 0;
   uint32_t launches = 0;
   float last_ms = 0;
+  uint32_t last_chunks = 0;            // the last batch: chunks it ran as, whether orphan rescue ran (candidate tap)
+  int last_rescue = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   // finished result (host)
   std::vector<uint64_t> h_off, h_counts;
@@ -1702,6 +1704,8 @@ static int map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, u
   }
   c->frag_counter += h.mapped;
   c->frags_seen += n;
+  c->last_chunks = nch;
+  c->last_rescue = p.recover_orphans && !single_end;
   c->timestep += nsteps;
   c->full_dp_total += full_dp;
   c->rescued_total += rctr[0]; c->rescue_searches_total += rctr[1]; c->rescue_no_room_total += rctr[2];
@@ -1866,6 +1870,27 @@ extern "C" int sb_map_last_alignments(sb_map_ctx* c, uint32_t n, uint32_t* n_aln
   if (flen) SB_CUDA(cudaMemcpy(flen, b.flen, n * cap * 4, cudaMemcpyDeviceToHost));
   if (label) SB_CUDA(cudaMemcpy(label, b.label, n * 2 * cap * 4, cudaMemcpyDeviceToHost));
   if (weight) SB_CUDA(cudaMemcpy(weight, b.weight, n * cap * 8, cudaMemcpyDeviceToHost));
+  return SB_OK;
+}
+
+// parity tap: per-read candidates of the LAST batch as the seed kernel left them (n_l / n_r [n], cand_l / cand_r
+// [n * MAXCAND]; bit 31 of n_l marks a read the seed kernel found unmapped).  The candidate buffers hold one chunk (and
+// alternate between two sets from chunk to chunk), and orphan rescue appends to them: such batches are refused.
+extern "C" int sb_map_last_candidates(sb_map_ctx* c, uint32_t n, uint32_t* n_l, uint32_t* n_r, void* cand_l,
+                                      void* cand_r) {
+  if (!c) { sb::set_error("null argument"); return SB_ERR_INVALID; }
+  if (c->last_chunks > 1 || c->last_rescue) {
+    sb::set_error("sb_map_last_candidates: the last batch ran as %u chunks%s; candidates are kept for one chunk without "
+                  "orphan rescue", c->last_chunks, c->last_rescue ? " with orphan rescue" : "");
+    return SB_ERR_STATE;
+  }
+  if (n > c->chunk_cap) { sb::set_error("sb_map_last_candidates: %u reads, the buffers hold %u", n, c->chunk_cap); return SB_ERR_INVALID; }
+  SB_CUDA(cudaSetDevice(c->device));
+  const BatchBufs& b = c->b;
+  if (n_l) SB_CUDA(cudaMemcpy(n_l, b.n_l, (size_t)n * 4, cudaMemcpyDeviceToHost));
+  if (n_r) SB_CUDA(cudaMemcpy(n_r, b.n_r, (size_t)n * 4, cudaMemcpyDeviceToHost));
+  if (cand_l) SB_CUDA(cudaMemcpy(cand_l, b.cand_l, (size_t)n * MAXCAND * sizeof(Cand), cudaMemcpyDeviceToHost));
+  if (cand_r) SB_CUDA(cudaMemcpy(cand_r, b.cand_r, (size_t)n * MAXCAND * sizeof(Cand), cudaMemcpyDeviceToHost));
   return SB_OK;
 }
 

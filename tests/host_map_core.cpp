@@ -129,6 +129,24 @@ extern "C" int hmc_map_throughput(uint32_t n_txps, uint32_t k, const uint64_t* t
   return 0;
 }
 
+// the product's serial seed / chain form on one mate (tests/test_seed_paths_cpu.py): candidates in (tid, ori, diag_c)
+// order, counters3 = {lookups, postings, seeds} of this mate
+extern "C" uint32_t hmc_mate_candidates(uint32_t n_txps, uint32_t k, const uint64_t* tx_off, const uint8_t* codes,
+                                        const void* table, uint64_t table_capacity, const void* postings, const Params* p,
+                                        const uint8_t* read, uint32_t L, Cand* out /* [MAXCAND] */,
+                                        unsigned long long* counters3) {
+  IndexView ix;
+  ix.n_txps = n_txps; ix.k = k; ix.mask = table_capacity - 1; ix.tx_off = tx_off; ix.codes = codes;
+  ix.table = (const TableEntry*)table; ix.post = (const Posting*)postings;
+  ix.packed = nullptr; ix.tx_has_n = nullptr;
+  std::vector<uint64_t> keys(MAXSEEDS);
+  Counters ctr;
+  memset(&ctr, 0, sizeof(ctr));
+  const uint32_t n = mate_candidates(ix, *p, read, L, keys.data(), 1, out, ctr);
+  counters3[0] = ctr.lookups; counters3[1] = ctr.postings; counters3[2] = ctr.seeds;
+  return n;
+}
+
 // the product's serial DP form on one reference (tests/test_dp_vs_edlib.py)
 extern "C" int32_t hmc_dp_score(const uint64_t* tx_off, const uint8_t* codes, const Params* p, const uint8_t* read, uint32_t L,
                                 uint32_t ori, uint32_t tid, int32_t diag_c) {

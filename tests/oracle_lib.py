@@ -355,3 +355,25 @@ class Online:
             load().orc_online_free(self.h)
         except Exception:
             pass
+
+
+class orc_mate_info(C.Structure):
+    _fields_ = [(k, C.c_uint32) for k in ("lookups", "postings_all", "seeds", "cut_round", "distinct", "chains",
+                                          "survivors", "straddle_seeds", "straddle_distinct")]
+
+    def asdict(self):
+        return {k: int(getattr(self, k)) for k, _ in self._fields_}
+
+
+ORC_CAND_DTYPE = np.dtype([("tid", np.uint32), ("ori", np.uint32), ("diag_c", np.int32), ("cov", np.uint32)])
+
+
+def mate_candidates(index, p, read):
+    """orc_mate_candidates: the candidates of one mate (structured array of ORC_CAND_DTYPE) and what its seeds look
+    like (orc_mate_info as a dict)"""
+    lib = load()
+    read = np.ascontiguousarray(read, dtype=np.uint8)
+    out = np.zeros(64, ORC_CAND_DTYPE)
+    info = orc_mate_info()
+    n = lib.orc_mate_candidates(index.h, C.byref(p), _p(read), C.c_uint32(read.shape[0]), _p(out), C.byref(info))
+    return out[:n].copy(), info.asdict()

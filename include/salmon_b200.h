@@ -110,6 +110,7 @@ int sb_em_optimize(sb_em_ctx* ctx, const sb_eq_csr* eq, const sb_em_params* p,
 int sb_em_upload(sb_em_ctx* ctx, const sb_eq_csr* eq,
                  const double* projected_counts, const double* eff_len,
                  const uint64_t* unique_counts);
+/* sb_em_prepare refuses (SB_ERR_INVALID) a negative or non-finite vb_prior. */
 int sb_em_prepare(sb_em_ctx* ctx, const sb_em_params* p, sb_em_stats* stats);
 int sb_em_run(sb_em_ctx* ctx, sb_em_stats* stats);   /* re-runnable: restarts from the prepared state */
 int sb_em_download(sb_em_ctx* ctx, double* alpha_out, sb_em_stats* stats);
@@ -648,7 +649,8 @@ int sb_em_set_option(sb_em_ctx* ctx, const char* key, int64_t value);
  * suffix "_cm" (class-major) / "_tm" (transcript-major): "stream_bytes", "sell_cols" (SELL columns of 32 entries),
  * "long_rows", "long_entries", "fallback_rows" (rows on the long-row path only because their slice's indices span
  * more than 16 bits); "warps" (warps of the iteration grid, which the slice ranges were cut for), "ring_cols" (columns
- * one warp's stream ring holds). */
+ * one warp's stream ring holds), "sum_scale_log2" (s: the iteration sums alpha' + prior in fixed point, in units
+ * of 2^-s; 20, or less when the class counts and priors are large enough to need it). */
 int sb_em_get_info(sb_em_ctx* ctx, const char* key, int64_t* value);
 
 /* ---- multi-GPU: classes stay sharded per rank, alpha is all-reduced once per

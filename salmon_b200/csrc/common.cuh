@@ -154,8 +154,10 @@ __device__ __forceinline__ double digamma_1_2(double x) {
   const double r = p / q;
   return g * Y + g * r;
 }
-// x > 0 only (callers guard with digammaMin = 1e-10).
+// x > 0 only (callers guard with digammaMin = 1e-10).  Anything else (x <= 0, NaN) returns NaN at once: the upward
+// recurrence below would otherwise run |x| times.
 __device__ __forceinline__ double digamma_pos(double x) {
+  if (!(x > 0.0)) return __longlong_as_double(0x7ff8000000000000ll);
   if (x >= 10.0) return digamma_large(x);
   double result = 0.0;
   while (x > 2.0) {

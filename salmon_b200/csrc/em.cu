@@ -23,6 +23,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <string>
 #include <vector>
 
@@ -587,6 +588,8 @@ extern "C" int sb_em_get_info(sb_em_ctx* c, const char* key, int64_t* value) {
   // warps of the grid the slice ranges were cut for, and the columns one warp's ring holds
   if (!strcmp(key, "warps")) { *value = (int64_t)c->grid * (EM_THREADS / 32); return SB_OK; }
   if (!strcmp(key, "ring_cols")) { *value = (int64_t)EM_CH * EM_RING; return SB_OK; }
+  // s of the fixed-point sum of (alpha' + prior): units of 2^-s, 20 unless the counts and priors are large
+  if (!strcmp(key, "sum_scale_log2")) { *value = c->sum_scale_log2; return SB_OK; }
   const size_t n = strlen(key);
   const SellDev* m = nullptr;
   if (n > 3 && !strcmp(key + n - 3, "_cm")) m = &c->cm;
@@ -643,6 +646,12 @@ extern "C" int sb_em_upload(sb_em_ctx* c, const sb_eq_csr* eq, const double* pro
   double tw = 0.0;
   for (uint32_t i = 0; i < M; ++i) tw += projected[i];
   c->total_weight = tw;
+  // inputs of the bound on sum(alpha' + prior) that sb_em_prepare scales the fixed-point sum by
+  double cs = 0.0, es = 0.0;
+  for (uint64_t k = 0; k < C; ++k) cs += (double)eq->counts[k];
+  for (uint32_t i = 0; i < M; ++i) es += fabs(eff_len[i]);
+  c->count_sum = cs;
+  c->eff_abs_sum = es;
   c->h2d_bytes = (C + 1) * 8 + C * 8 + nnz * 12 + (size_t)M * 24;
   SB_CUDA(cudaStreamSynchronize(st));
   c->uploaded = true;
@@ -763,6 +772,26 @@ static int em_rebalance(sb_em_ctx* c);
 extern "C" int sb_em_prepare(sb_em_ctx* c, const sb_em_params* p, sb_em_stats* stats) {
   if (!c || !p) { set_error("null argument"); return SB_ERR_INVALID; }
   if (!c->uploaded) { set_error("sb_em_prepare before sb_em_upload"); return SB_ERR_STATE; }
+  if (!(p->vb_prior >= 0.0) || !std::isfinite(p->vb_prior)) {
+    set_error("the VB prior (--vbPrior) must be a finite number >= 0, not %g", p->vb_prior);
+    return SB_ERR_INVALID;
+  }
+  // Unit of P2's fixed-point sum of (alpha' + prior) over the active rows (em_kernels.cuh: P2Acc).  An iteration's
+  // alpha' add up to the counts of the classes it keeps, plus 1.0 per transcript in the first plain-EM iteration; the
+  // priors add vb_prior per transcript or per unit of effective length.  Twice that bound B leaves room for rounding,
+  // and the largest s <= 20 with 2B * 2^s < 2^62 keeps every row's term and the grid's total inside 64 bits.
+  {
+    const double prior_sum = p->per_txp_prior ? p->vb_prior * (double)c->M
+                                              : p->vb_prior * (p->no_length_correction ? 100.0 * (double)c->M : c->eff_abs_sum);
+    const double bound = 2.0 * (c->count_sum + (double)c->M + prior_sum);
+    if (!std::isfinite(bound)) {
+      set_error("the class counts and priors sum to %g, which the EM cannot represent", bound);
+      return SB_ERR_INVALID;
+    }
+    int e2 = 0;
+    frexp(bound, &e2);   // bound < 2^e2
+    c->sum_scale_log2 = std::min(20, 62 - e2);
+  }
   SB_CUDA(cudaSetDevice(c->device));
   cudaStream_t st = c->stream;
   c->params = *p;
@@ -1016,6 +1045,7 @@ static void fill_args(sb_em_ctx* c, EmArgs& A, bool row_space) {
   A.maxrel = (unsigned long long*)(c->d_scalars + 24);
   A.inactive_sum = ov ? c->ov_inactive_sum : c->inactive_sum;
   A.sum0 = ov ? c->ov_sum0 : c->sum0;
+  A.sum_scale = ldexp(1.0, c->sum_scale_log2);
   A.min_eq_w = ov ? c->ov_min_eq_w : DBL_MIN;
   A.first_bias = ov ? 0.0 : (c->params.use_vbem ? 0.0 : 1.0);
   A.tol = c->params.tol; A.min_iter = c->params.min_iter; A.max_iter = c->params.max_iter;

@@ -50,6 +50,8 @@ struct sb_em_ctx {
   uint64_t C = 0, nnz = 0;
   uint32_t M = 0;
   double total_weight = 0.0;
+  double count_sum = 0.0, eff_abs_sum = 0.0;   // sum of the class counts, of |effective length|
+  int sum_scale_log2 = 20;                     // the fixed-point sum of (alpha' + prior) counts units of 2^-s
   size_t h2d_bytes = 0;
   bool uploaded = false, prepared = false;
   sb_em_params params{};

@@ -87,6 +87,7 @@ struct EmArgs {
   double* sum_partial;          // [2][grid]
   unsigned long long* maxrel;   // [2] bit pattern of a non-negative double
   double inactive_sum; double sum0;
+  double sum_scale;             // 2^s: unit of the fixed-point sum of (alpha' + prior), chosen at prepare (P2Acc)
   double tol;
   double min_eq_w;              // denominator guard: DBL_MIN (optimize) / denorm_min (serial EM)
   double first_bias;            // 1.0 for optimize's first plain-EM iteration (:812,:821), else 0
@@ -132,11 +133,11 @@ __device__ __forceinline__ unsigned long long gtime_ns() {
   return t;
 }
 
-// sum of (alpha' + prior) over my rows, in units of 2^-20: integer additions commute, so the total -- and with it
-// logNorm and every later bit of the run -- does not depend on which warp took which row (dynamic long-row queue) or
-// on how the ranges were cut (measured re-balancing): runs are bit-reproducible.  (logNorm only has to be the same
-// everywhere: any common factor of theta cancels in P1/P2.)
-constexpr double SUM_FIXED = 1048576.0;
+// sum of (alpha' + prior) over my rows, in units of 1 / A.sum_scale (2^-20 unless the table is large): integer
+// additions commute, so the total -- and with it logNorm and every later bit of the run -- does not depend on which
+// warp took which row (dynamic long-row queue) or on how the ranges were cut (measured re-balancing): runs are
+// bit-reproducible.  (logNorm only has to be the same everywhere: any common factor of theta cancels in P1/P2.)
+// sb_em_prepare picks the scale so that the grid's total stays below 2^62 (em.cu: sum_scale_log2).
 struct P2Acc {
   long long isum;
   double maxrel;  // max rel diff over my rows
@@ -250,7 +251,7 @@ __device__ __forceinline__ void row_finish(const EmArgs& A, uint32_t row, const 
     if (na > ALPHA_CHECK_CUTOFF) pa.maxrel = fmax(pa.maxrel, fabs(o.x3 - na) / na);
     A.alpha[row] = na;
     const double ap = na + pr;
-    pa.isum += __double2ll_rn(ap * SUM_FIXED);
+    pa.isum += __double2ll_rn(ap * A.sum_scale);
     A.theta[row] = theta_of<VBEM>(na, ap, logNorm);
   } else {
     const uint32_t t = (uint32_t)__double_as_longlong(o.x3);
@@ -614,7 +615,7 @@ __device__ __forceinline__ void lag_lognorm_warp0(const EmArgs& A, uint32_t par,
     long long acc = 0;
     for (uint32_t i = threadIdx.x; i < nblk; i += 32) acc += __double_as_longlong(__ldcg(&part[i]));
     acc = warp_sum_ll(acc);
-    if (threadIdx.x == 0) scratch[33] = digamma_pos((double)acc / SUM_FIXED + A.inactive_sum);
+    if (threadIdx.x == 0) scratch[33] = digamma_pos((double)acc / A.sum_scale + A.inactive_sum);
   }
 }
 

@@ -637,6 +637,11 @@ int sb_reads_bucketed_meta(sb_reads* rd, uint32_t min_len, uint32_t batch, uint3
  * Returns the number of warps (call with out=NULL to size the buffer). */
 int sb_em_debug_timeline(sb_em_ctx* ctx, uint64_t* out, uint32_t iteration);
 
+/* Debug: the library's CUDA resources, process-wide: out3 = {live buffers, streams and events; live buffer bytes;
+ * buffers, streams and events made since the library was loaded}.  Leaks and reallocations show here even on a GPU
+ * that other processes share. */
+int sb_debug_device_memory(uint64_t out3[3]);
+
 /* Tuning knobs (not part of the reference contract).  Unknown keys return SB_ERR_INVALID.
  * key: "variant" (0 = multi-kernel per iteration, 1 = persistent cooperative), "blocks_per_sm" (0 = as many as fit),
  *      "sell_group_cm" / "sell_group_tm" (rows per length-bucketing group, a power of two >= 32), "rebalance" (rounds

@@ -205,6 +205,7 @@ SYMBOLS = {
     "sb_em_set_option": (C.c_int, [_P, C.c_char_p, C.c_int64]),
     "sb_em_get_info": (C.c_int, [_P, C.c_char_p, C.POINTER(C.c_int64)]),
     "sb_em_debug_timeline": (C.c_int, [_P, _P, C.c_uint32]),
+    "sb_debug_device_memory": (C.c_int, [_P]),
     "sb_bootstrap": (C.c_int, [_P, C.POINTER(sb_em_params), C.c_double, C.c_uint32, C.c_uint64, _P, _P]),
     "sb_bootstrap_last_counts": (C.c_int, [_P, _P]),
     "sb_gibbs": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_double, C.c_uint32, C.c_uint32, C.c_int, C.c_double,

@@ -456,32 +456,6 @@ extern "C" void sb_em_default_params(sb_em_params* p) {
   p->max_iter = 10000;
 }
 
-// Grow-only device buffers: capacity is remembered per pointer slot so that repeated
-// optimize() calls on same-sized problems never touch cudaMalloc/cudaFree again.
-#include <unordered_map>
-static std::unordered_map<void**, size_t>& cap_table() {
-  static thread_local std::unordered_map<void**, size_t> t;
-  return t;
-}
-template <typename T>
-static int dev_alloc(T** p, size_t n) {
-  if (n == 0) n = 1;
-  const size_t bytes = n * sizeof(T);
-  auto& caps = cap_table();
-  auto it = caps.find((void**)p);
-  if (*p && it != caps.end() && it->second >= bytes) return SB_OK;
-  if (*p) { cudaFree(*p); *p = nullptr; }
-  const size_t want = bytes + bytes / 16 + 256;  // a little slack against small size changes
-  cudaError_t e = cudaMalloc((void**)p, want);
-  if (e != cudaSuccess) {
-    set_error("cudaMalloc(%zu bytes) failed: %s", want, cudaGetErrorString(e));
-    caps.erase((void**)p);
-    return SB_ERR_NOMEM;
-  }
-  caps[(void**)p] = want;
-  return SB_OK;
-}
-
 extern "C" sb_em_ctx* sb_em_create(int device) {
   int n = sb_device_count();
   if (n <= 0) {
@@ -492,62 +466,22 @@ extern "C" sb_em_ctx* sb_em_create(int device) {
     set_error("device %d out of range (0..%d)", device, n - 1);
     return nullptr;
   }
-  sb_em_ctx* c = new sb_em_ctx();
-  c->device = device;
-  if (cudaSetDevice(device) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) {
+  if (cudaSetDevice(device) != cudaSuccess) {
     set_error("cannot initialise device %d: %s", device, cudaGetErrorString(cudaGetLastError()));
-    delete c;
     return nullptr;
   }
+  sb_em_ctx* c = new sb_em_ctx(device);
+  int rc = c->res.stream(&c->stream, cudaStreamNonBlocking);
+  for (int i = 0; i < 4 && rc == SB_OK; ++i) rc = c->res.event(&c->ev[i], cudaEventDefault);
+  if (rc != SB_OK) { delete c; return nullptr; }
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device);
   c->n_sm = prop.multiProcessorCount;
   c->l2_bytes = (size_t)prop.l2CacheSize;
-  for (int i = 0; i < 4; ++i) cudaEventCreate(&c->ev[i]);
   // development overrides of the tuning defaults (sweeps over the test-suite)
   if (const char* e = getenv("SB_EM_GROUP_CM")) { const int v = atoi(e); if (v >= 32 && !(v & (v - 1))) c->sell_group_cm = v; }
   if (const char* e = getenv("SB_EM_GROUP_TM")) { const int v = atoi(e); if (v >= 32 && !(v & (v - 1))) c->sell_group_tm = v; }
   return c;
-}
-
-static void free_sell(SellDev& m) {
-  void** ptrs[] = {(void**)&m.slice_ptr, (void**)&m.width, (void**)&m.base, (void**)&m.len, (void**)&m.idx,
-                   (void**)&m.w, (void**)&m.warp_begin, (void**)&m.long_rows};
-  for (void** p : ptrs) {
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    cap_table().erase(p);
-  }
-}
-static void free_all(sb_em_ctx* c) {
-  void** ptrs[] = {(void**)&c->d_off, (void**)&c->d_tids, (void**)&c->d_aux, (void**)&c->d_counts,
-                   (void**)&c->d_projected, (void**)&c->d_eff_in, (void**)&c->d_unique,
-                   (void**)&c->d_efflens, (void**)&c->d_prior, (void**)&c->d_alpha0,
-                   (void**)&c->d_alpha, (void**)&c->d_theta, (void**)&c->d_base, (void**)&c->d_cw,
-                   (void**)&c->d_packed, (void**)&c->d_packed2, (void**)&c->d_packed_scan,
-                   (void**)&c->d_valid, (void**)&c->d_scalars, (void**)&c->d_tcnt,
-                   (void**)&c->d_tid_row, (void**)&c->m_off, (void**)&c->m_idx,
-                   (void**)&c->m_idx_state, (void**)&c->m_w, (void**)&c->t_off, (void**)&c->t_idx,
-                   (void**)&c->t_w, (void**)&c->d_cnt, (void**)&c->d_scale, (void**)&c->d_ent_cls,
-                   (void**)&c->d_row_tid, (void**)&c->d_rank_tid, (void**)&c->d_rowperm,
-                   (void**)&c->d_order, (void**)&c->d_sort_keys, (void**)&c->d_sort_vals,
-                   (void**)&c->d_sort_keys2, (void**)&c->d_sort_vals2, (void**)&c->d_tmp,
-                   (void**)&c->d_sum_partial, (void**)&c->d_flush, (void**)&c->d_part,
-                   (void**)&c->d_part_red, (void**)&c->r_alpha, (void**)&c->r_theta,
-                   (void**)&c->r_prior, (void**)&c->r_base, (void**)&c->r_alpha0,
-                   (void**)&c->d_dbg, (void**)&c->d_cdf, (void**)&c->d_cls_map, (void**)&c->d_samp,
-                   (void**)&c->d_valid_boot, (void**)&c->d_active, (void**)&c->d_gibbs_cnt,
-                   (void**)&c->d_gibbs_mu, (void**)&c->d_gibbs_prior, (void**)&c->d_gibbs_out,
-                   (void**)&c->ov_cnt, (void**)&c->ov_base_row, (void**)&c->ov_base_tid,
-                   (void**)&c->ov_alpha0_row, (void**)&c->ov_alpha0_tid};
-  for (void** p : ptrs) {
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    cap_table().erase(p);
-  }
-  free_sell(c->cm);
-  free_sell(c->tm);
 }
 
 extern "C" void sb_em_destroy(sb_em_ctx* c) {
@@ -555,11 +489,7 @@ extern "C" void sb_em_destroy(sb_em_ctx* c) {
   cudaSetDevice(c->device);
   cudaDeviceSynchronize();
   for (void* p : c->x_opened) cudaIpcCloseMemHandle(p);
-  cudaFree(c->x_block); cudaFree(c->d_peers); cudaFree(c->d_xfail);
   sb_em_comm_destroy(c);
-  free_all(c);
-  for (int i = 0; i < 4; ++i) cudaEventDestroy(c->ev[i]);
-  cudaStreamDestroy(c->stream);
   delete c;
 }
 
@@ -620,13 +550,13 @@ extern "C" int sb_em_upload(sb_em_ctx* c, const sb_eq_csr* eq, const double* pro
   if (nnz && (!eq->tids || !eq->weights)) { set_error("null CSR arrays"); return SB_ERR_INVALID; }
   c->C = C; c->M = M; c->nnz = nnz;
   c->prepared = false;
-  SB_TRY(dev_alloc(&c->d_off, C + 1));
-  SB_TRY(dev_alloc(&c->d_tids, nnz));
-  SB_TRY(dev_alloc(&c->d_aux, nnz));
-  SB_TRY(dev_alloc(&c->d_counts, C));
-  SB_TRY(dev_alloc(&c->d_projected, M));
-  SB_TRY(dev_alloc(&c->d_eff_in, M));
-  SB_TRY(dev_alloc(&c->d_unique, M));
+  SB_TRY(c->res.grow(&c->d_off, C + 1));
+  SB_TRY(c->res.grow(&c->d_tids, nnz));
+  SB_TRY(c->res.grow(&c->d_aux, nnz));
+  SB_TRY(c->res.grow(&c->d_counts, C));
+  SB_TRY(c->res.grow(&c->d_projected, M));
+  SB_TRY(c->res.grow(&c->d_eff_in, M));
+  SB_TRY(c->res.grow(&c->d_unique, M));
   cudaStream_t st = c->stream;
   if (C) {
     SB_CUDA(cudaMemcpyAsync(c->d_off, eq->off, (C + 1) * 8, cudaMemcpyHostToDevice, st));
@@ -702,11 +632,11 @@ static int build_sell(sb_em_ctx* c, SellDev& m, uint32_t n_rows, const uint32_t*
   m.csr_idx = csr_idx;
   m.csr_w = csr_w;
   m.zero = pad_idx;
-  SB_TRY(dev_alloc(&m.len, (size_t)n_rows));
-  SB_TRY(dev_alloc(&m.width, (size_t)m.n_slices + 1));
-  SB_TRY(dev_alloc(&m.slice_ptr, (size_t)m.n_slices + 1));
-  SB_TRY(dev_alloc(&m.base, (size_t)m.n_slices + 1));
-  SB_TRY(dev_alloc(&m.warp_begin, (size_t)n_warps + 1));
+  SB_TRY(c->res.grow(&m.len, (size_t)n_rows));
+  SB_TRY(c->res.grow(&m.width, (size_t)m.n_slices + 1));
+  SB_TRY(c->res.grow(&m.slice_ptr, (size_t)m.n_slices + 1));
+  SB_TRY(c->res.grow(&m.base, (size_t)m.n_slices + 1));
+  SB_TRY(c->res.grow(&m.warp_begin, (size_t)n_warps + 1));
   uint32_t* d_nlong = (uint32_t*)(c->d_scalars + 8);   // [0] long rows, [1] fill cursor, [2] fallback rows
   SB_CUDA(cudaMemsetAsync(d_nlong, 0, 16, st));
   SB_CUDA(cudaMemsetAsync(m.width, 0, ((size_t)m.n_slices + 1) * 4, st));
@@ -726,9 +656,9 @@ static int build_sell(sb_em_ctx* c, SellDev& m, uint32_t n_rows, const uint32_t*
   SB_CUDA(cudaMemcpyAsync(&m.n_fallback, d_nlong + 2, 4, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaStreamSynchronize(st));
   m.n_cols = ncols;
-  SB_TRY(dev_alloc(&m.idx, (size_t)ncols * 32 + 32));
-  SB_TRY(dev_alloc(&m.w, (size_t)ncols * 32 + 32));
-  SB_TRY(dev_alloc(&m.long_rows, (size_t)3 * m.n_long + 3));
+  SB_TRY(c->res.grow(&m.idx, (size_t)ncols * 32 + 32));
+  SB_TRY(c->res.grow(&m.w, (size_t)ncols * 32 + 32));
+  SB_TRY(c->res.grow(&m.long_rows, (size_t)3 * m.n_long + 3));
   SB_CUDA(cudaMemsetAsync(m.idx, 0xff, ((size_t)ncols * 32 + 32) * 2, st));
   SB_CUDA(cudaMemsetAsync(m.w, 0, ((size_t)ncols * 32 + 32) * 8, st));
   if (m.n_slices) {
@@ -822,27 +752,27 @@ extern "C" int sb_em_prepare(sb_em_ctx* c, const sb_em_params* p, sb_em_stats* s
 
   const uint64_t NP = std::max<uint64_t>(C, M) + 1;
   const uint64_t NS = std::max<uint64_t>(std::max<uint64_t>(C, nnz), (uint64_t)M) + 1;
-  SB_TRY(dev_alloc(&c->d_efflens, M));
-  SB_TRY(dev_alloc(&c->d_prior, M));
-  SB_TRY(dev_alloc(&c->d_alpha0, M));
-  SB_TRY(dev_alloc(&c->d_alpha, M));
-  SB_TRY(dev_alloc(&c->d_theta, (size_t)M + 4));
+  SB_TRY(c->res.grow(&c->d_efflens, M));
+  SB_TRY(c->res.grow(&c->d_prior, M));
+  SB_TRY(c->res.grow(&c->d_alpha0, M));
+  SB_TRY(c->res.grow(&c->d_alpha, M));
+  SB_TRY(c->res.grow(&c->d_theta, (size_t)M + 4));
   SB_CUDA(cudaMemsetAsync(c->d_theta, 0, ((size_t)M + 4) * 8, st));
-  SB_TRY(dev_alloc(&c->d_base, M));
-  SB_TRY(dev_alloc(&c->d_cw, nnz));
-  SB_TRY(dev_alloc(&c->d_packed, NP));
-  SB_TRY(dev_alloc(&c->d_packed2, NP));
-  SB_TRY(dev_alloc(&c->d_packed_scan, NP));
-  SB_TRY(dev_alloc(&c->d_valid, C));
-  SB_TRY(dev_alloc(&c->d_cls_map, C));
-  SB_TRY(dev_alloc(&c->d_scalars, 64));
-  SB_TRY(dev_alloc(&c->d_tcnt, M));
-  SB_TRY(dev_alloc(&c->d_tid_row, M));
-  SB_TRY(dev_alloc(&c->d_sort_keys, NS));
-  SB_TRY(dev_alloc(&c->d_sort_vals, NS));
-  SB_TRY(dev_alloc(&c->d_sort_keys2, NS));
-  SB_TRY(dev_alloc(&c->d_sort_vals2, NS));
-  SB_TRY(dev_alloc(&c->d_order, NS));
+  SB_TRY(c->res.grow(&c->d_base, M));
+  SB_TRY(c->res.grow(&c->d_cw, nnz));
+  SB_TRY(c->res.grow(&c->d_packed, NP));
+  SB_TRY(c->res.grow(&c->d_packed2, NP));
+  SB_TRY(c->res.grow(&c->d_packed_scan, NP));
+  SB_TRY(c->res.grow(&c->d_valid, C));
+  SB_TRY(c->res.grow(&c->d_cls_map, C));
+  SB_TRY(c->res.grow(&c->d_scalars, 64));
+  SB_TRY(c->res.grow(&c->d_tcnt, M));
+  SB_TRY(c->res.grow(&c->d_tid_row, M));
+  SB_TRY(c->res.grow(&c->d_sort_keys, NS));
+  SB_TRY(c->res.grow(&c->d_sort_vals, NS));
+  SB_TRY(c->res.grow(&c->d_sort_keys2, NS));
+  SB_TRY(c->res.grow(&c->d_sort_vals2, NS));
+  SB_TRY(c->res.grow(&c->d_order, NS));
   SB_CUDA(cudaMemsetAsync(c->d_base, 0, (size_t)M * 8, st));
   SB_CUDA(cudaMemsetAsync(c->d_scalars, 0, 64 * 8, st));
   SB_CUDA(cudaMemsetAsync(c->d_tcnt, 0, (size_t)M * 4, st));
@@ -857,7 +787,7 @@ extern "C" int sb_em_prepare(sb_em_ctx* c, const sb_em_params* p, sb_em_stats* s
   }
   size_t need = std::max(t1, t2);
   if (need > c->tmp_bytes) {
-    SB_TRY(dev_alloc((unsigned char**)&c->d_tmp, need));
+    SB_TRY(c->res.grow((unsigned char**)&c->d_tmp, need));
     c->tmp_bytes = need;
   }
 
@@ -894,13 +824,13 @@ extern "C" int sb_em_prepare(sb_em_ctx* c, const sb_em_params* p, sb_em_stats* s
   c->n_cls = Cm; c->nnzm = nnzm;
 
   // compact class-major CSR in final class order
-  SB_TRY(dev_alloc(&c->m_off, (size_t)Cm + 1));
-  SB_TRY(dev_alloc(&c->m_idx, (size_t)nnzm + 1));
-  SB_TRY(dev_alloc(&c->m_idx_state, (size_t)nnzm + 1));
-  SB_TRY(dev_alloc(&c->m_w, (size_t)nnzm + 1));
-  SB_TRY(dev_alloc(&c->d_cnt, (size_t)Cm));
-  SB_TRY(dev_alloc(&c->d_scale, (size_t)Cm + 4));
-  SB_TRY(dev_alloc(&c->d_ent_cls, (size_t)nnzm));
+  SB_TRY(c->res.grow(&c->m_off, (size_t)Cm + 1));
+  SB_TRY(c->res.grow(&c->m_idx, (size_t)nnzm + 1));
+  SB_TRY(c->res.grow(&c->m_idx_state, (size_t)nnzm + 1));
+  SB_TRY(c->res.grow(&c->m_w, (size_t)nnzm + 1));
+  SB_TRY(c->res.grow(&c->d_cnt, (size_t)Cm));
+  SB_TRY(c->res.grow(&c->d_scale, (size_t)Cm + 4));
+  SB_TRY(c->res.grow(&c->d_ent_cls, (size_t)nnzm));
   SB_CUDA(cudaMemsetAsync(c->d_scale, 0, ((size_t)Cm + 4) * 8, st));
   SB_CUDA(cudaMemcpyAsync(c->m_off + Cm, &nnzm, 4, cudaMemcpyHostToDevice, st));
   if (C) {
@@ -929,18 +859,18 @@ extern "C" int sb_em_prepare(sb_em_ctx* c, const sb_em_params* p, sb_em_stats* s
     return SB_ERR_STATE;
   }
   c->n_rows = R;
-  SB_TRY(dev_alloc(&c->t_off, (size_t)R + 1));
-  SB_TRY(dev_alloc(&c->t_idx, (size_t)nnzm + 1));
-  SB_TRY(dev_alloc(&c->t_w, (size_t)nnzm + 1));
-  SB_TRY(dev_alloc(&c->d_rank_tid, (size_t)R + 1));
-  SB_TRY(dev_alloc(&c->d_rowperm, (size_t)R + 1));
-  SB_TRY(dev_alloc(&c->d_row_tid, (size_t)R + 1));
-  SB_TRY(dev_alloc(&c->r_alpha, (size_t)R + 1));
-  SB_TRY(dev_alloc(&c->r_theta, (size_t)R + 4));
+  SB_TRY(c->res.grow(&c->t_off, (size_t)R + 1));
+  SB_TRY(c->res.grow(&c->t_idx, (size_t)nnzm + 1));
+  SB_TRY(c->res.grow(&c->t_w, (size_t)nnzm + 1));
+  SB_TRY(c->res.grow(&c->d_rank_tid, (size_t)R + 1));
+  SB_TRY(c->res.grow(&c->d_rowperm, (size_t)R + 1));
+  SB_TRY(c->res.grow(&c->d_row_tid, (size_t)R + 1));
+  SB_TRY(c->res.grow(&c->r_alpha, (size_t)R + 1));
+  SB_TRY(c->res.grow(&c->r_theta, (size_t)R + 4));
   SB_CUDA(cudaMemsetAsync(c->r_theta, 0, ((size_t)R + 4) * 8, st));
-  SB_TRY(dev_alloc(&c->r_prior, (size_t)R + 1));
-  SB_TRY(dev_alloc(&c->r_base, (size_t)R + 1));
-  SB_TRY(dev_alloc(&c->r_alpha0, (size_t)R + 1));
+  SB_TRY(c->res.grow(&c->r_prior, (size_t)R + 1));
+  SB_TRY(c->res.grow(&c->r_base, (size_t)R + 1));
+  SB_TRY(c->res.grow(&c->r_alpha0, (size_t)R + 1));
   SB_CUDA(cudaMemcpyAsync(c->t_off + R, &nnzm, 4, cudaMemcpyHostToDevice, st));
   // rank_packed reuses d_packed2 (class packing no longer needed)
   k_rank_fill<<<nblk(M, 256), 256, 0, st>>>(M, c->d_tcnt, c->d_packed_scan, c->t_off, c->d_rank_tid,
@@ -983,7 +913,7 @@ extern "C" int sb_em_prepare(sb_em_ctx* c, const sb_em_params* p, sb_em_stats* s
   c->launches += 2;
   SB_CUDA(cudaMemcpyAsync(&c->sum0, d_sum0, 8, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaMemcpyAsync(&c->inactive_sum, d_inact, 8, cudaMemcpyDeviceToHost, st));
-  SB_TRY(dev_alloc(&c->d_sum_partial, (size_t)2 * std::max<uint32_t>(c->grid, 4096)));
+  SB_TRY(c->res.grow(&c->d_sum_partial, (size_t)2 * std::max<uint32_t>(c->grid, 4096)));
   SB_CUDA(cudaStreamSynchronize(st));
   c->prepared = true;
   // measured re-cut of the warp ranges (persistent kernels only: they carry the per-warp phase timers)
@@ -1117,50 +1047,38 @@ struct sb_comm {
   void* nccl = nullptr;
   cudaStream_t stream = nullptr;
   unsigned char* d_buf = nullptr;
-  size_t cap = 0;
+  sb::Resources res;
+  sb_comm(int rank_, int nranks_, int device_) : rank(rank_), nranks(nranks_), device(device_), res(device_) {}
 };
 extern "C" sb_comm* sb_comm_create(int rank, int nranks, const void* nccl_uid128, int device) {
   if (nranks < 1 || rank < 0 || rank >= nranks || (nranks > 1 && !nccl_uid128)) { set_error("sb_comm_create: bad arguments"); return nullptr; }
-  sb_comm* cm = new sb_comm();
-  cm->rank = rank; cm->nranks = nranks; cm->device = device;
-  if (nranks == 1) return cm;
-  if (nccl_load() != SB_OK) { delete cm; return nullptr; }
-  if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreate(&cm->stream) != cudaSuccess) {
-    set_error("sb_comm_create: cannot use device %d", device); delete cm; return nullptr;
-  }
+  if (nranks == 1) return new sb_comm(rank, nranks, device);
+  if (nccl_load() != SB_OK) return nullptr;
+  if (cudaSetDevice(device) != cudaSuccess) { set_error("sb_comm_create: cannot use device %d", device); return nullptr; }
+  sb_comm* cm = new sb_comm(rank, nranks, device);
+  if (cm->res.stream(&cm->stream, cudaStreamDefault) != SB_OK) { delete cm; return nullptr; }
   NcclUid u;
   memcpy(u.b, nccl_uid128, 128);
   const int r = g_nccl.CommInitRank(&cm->nccl, nranks, u, rank);
   if (r != 0) {
     set_error("ncclCommInitRank -> %d (%s)", r, g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?");
-    cudaStreamDestroy(cm->stream); delete cm; return nullptr;
+    delete cm; return nullptr;
   }
   return cm;
 }
 extern "C" void sb_comm_destroy(sb_comm* cm) {
   if (!cm) return;
   if (cm->nccl && g_nccl.CommDestroy) g_nccl.CommDestroy(cm->nccl);
-  if (cm->d_buf) { cudaSetDevice(cm->device); cudaFree(cm->d_buf); }
-  if (cm->stream) cudaStreamDestroy(cm->stream);
   delete cm;
 }
 extern "C" int sb_comm_rank(const sb_comm* cm) { return cm ? cm->rank : 0; }
 extern "C" int sb_comm_size(const sb_comm* cm) { return cm ? cm->nranks : 1; }
-static int comm_reserve(sb_comm* cm, size_t bytes) {
-  if (bytes <= cm->cap) return SB_OK;
-  SB_CUDA(cudaSetDevice(cm->device));
-  if (cm->d_buf) cudaFree(cm->d_buf);
-  cm->d_buf = nullptr; cm->cap = 0;
-  SB_CUDA(cudaMalloc(&cm->d_buf, bytes + 256));
-  cm->cap = bytes;
-  return SB_OK;
-}
 // in place over host buffers; dtype: 0 = f64, 1 = u64; op: 0 sum, 2 max, 3 min (ncclRedOp_t)
 extern "C" int sb_comm_allreduce(sb_comm* cm, void* buf, size_t n, int dtype, int op) {
   if (!cm || (n && !buf)) { set_error("null argument"); return SB_ERR_INVALID; }
   if (cm->nranks == 1 || n == 0) return SB_OK;
-  SB_TRY(comm_reserve(cm, n * 8));
   SB_CUDA(cudaSetDevice(cm->device));
+  SB_TRY(cm->res.grow(&cm->d_buf, n * 8));
   SB_CUDA(cudaMemcpyAsync(cm->d_buf, buf, n * 8, cudaMemcpyHostToDevice, cm->stream));
   SB_NCCL(g_nccl.AllReduce(cm->d_buf, cm->d_buf, n, dtype == 0 ? /*ncclFloat64*/ 8 : /*ncclUint64*/ 5, op, cm->nccl, cm->stream));
   SB_CUDA(cudaMemcpyAsync(buf, cm->d_buf, n * 8, cudaMemcpyDeviceToHost, cm->stream));
@@ -1172,8 +1090,8 @@ extern "C" int sb_comm_allgather(sb_comm* cm, const void* send, void* recv, size
   if (!cm || !send || !recv) { set_error("null argument"); return SB_ERR_INVALID; }
   if (cm->nranks == 1) { memcpy(recv, send, bytes); return SB_OK; }
   const size_t padded = (bytes + 15) & ~(size_t)15;
-  SB_TRY(comm_reserve(cm, padded * (size_t)(cm->nranks + 1)));
   SB_CUDA(cudaSetDevice(cm->device));
+  SB_TRY(cm->res.grow(&cm->d_buf, padded * (size_t)(cm->nranks + 1)));
   SB_CUDA(cudaMemcpyAsync(cm->d_buf, send, bytes, cudaMemcpyHostToDevice, cm->stream));
   SB_NCCL(g_nccl.AllGather(cm->d_buf, cm->d_buf + padded, padded, /*ncclInt8*/ 0, cm->nccl, cm->stream));
   std::vector<unsigned char> tmp(padded * (size_t)cm->nranks);
@@ -1223,12 +1141,18 @@ extern "C" int sb_em_peer_handle(sb_em_ctx* c, uint32_t max_txps, void* out64) {
   if (!c || !out64 || !max_txps) { set_error("null argument"); return SB_ERR_INVALID; }
   SB_CUDA(cudaSetDevice(c->device));
   if (c->x_block && c->x_cap < max_txps) { set_error("exchange block already allocated for %u transcripts", c->x_cap); return SB_ERR_STATE; }
-  if (!c->x_block) {
+  if (!c->x_block) {   // both buffers are made before either is recorded: a failure leaves the context as it was
     const size_t bytes = XchgLayout(max_txps, 64).bytes() + 64 * 8;   // G * ceil(M / G) <= M + 63 for every G <= 64
-    SB_CUDA(cudaMalloc(&c->x_block, bytes));
-    SB_CUDA(cudaMemset(c->x_block, 0, bytes));
-    SB_CUDA(cudaMalloc(&c->d_xfail, 4));
-    c->x_cap = max_txps;
+    unsigned char* xb = nullptr;
+    uint32_t* xf = nullptr;
+    int rc = c->res.alloc(&xb, bytes);
+    if (rc == SB_OK) rc = c->res.alloc(&xf, 1);
+    if (rc == SB_OK) {
+      const cudaError_t e = cudaMemset(xb, 0, bytes);
+      if (e != cudaSuccess) { set_error("clearing the exchange block: %s", cudaGetErrorString(e)); rc = SB_ERR_CUDA; }
+    }
+    if (rc != SB_OK) { c->res.release(xb); c->res.release(xf); return rc; }
+    c->x_block = xb; c->d_xfail = xf; c->x_cap = max_txps;
   }
   cudaIpcMemHandle_t h;
   SB_CUDA(cudaIpcGetMemHandle(&h, c->x_block));
@@ -1254,7 +1178,7 @@ extern "C" int sb_em_peer_open(sb_em_ctx* c, int rank, int nranks, const void* h
     ptrs[q] = (unsigned char*)p;
     c->x_opened.push_back(p);
   }
-  if (!c->d_peers) SB_CUDA(cudaMalloc(&c->d_peers, 64 * sizeof(unsigned char*)));
+  if (!c->d_peers) SB_TRY(c->res.alloc(&c->d_peers, 64));
   SB_CUDA(cudaMemcpy(c->d_peers, ptrs.data(), (size_t)nranks * sizeof(unsigned char*), cudaMemcpyHostToDevice));
   c->rank = rank; c->nranks = nranks;
   c->peers_ready = true;
@@ -1272,7 +1196,7 @@ static int em_run_multi_gpu_fused(sb_em_ctx* c, EmArgs& A, uint32_t* out,
   const int vb = c->params.use_vbem ? 1 : 0;
   const XchgLayout X(M, (uint32_t)c->nranks);
   SB_CUDA(cudaMemsetAsync(c->d_xfail, 0, 4, st));
-  SB_TRY(dev_alloc(&c->d_part, (size_t)M));
+  SB_TRY(c->res.grow(&c->d_part, (size_t)M));
   // locally inactive transcripts contribute their (constant) folded singleton mass
   SB_CUDA(cudaMemcpyAsync(c->d_part, c->d_base, (size_t)M * 8, cudaMemcpyDeviceToDevice, st));
   A.part_out = c->d_part;
@@ -1305,8 +1229,8 @@ static int em_run_multi_gpu(sb_em_ctx* c, EmArgs& A, uint32_t* out,
   const uint32_t M = c->M;
   const int vb = c->params.use_vbem ? 1 : 0;
   if (!c->nccl_comm) { set_error("multi-GPU EM: neither peers (sb_em_peer_open) nor NCCL (sb_em_comm_init) are set up"); return SB_ERR_STATE; }
-  SB_TRY(dev_alloc(&c->d_part, (size_t)M));
-  SB_TRY(dev_alloc(&c->d_part_red, (size_t)M));
+  SB_TRY(c->res.grow(&c->d_part, (size_t)M));
+  SB_TRY(c->res.grow(&c->d_part_red, (size_t)M));
   // locally inactive transcripts contribute their (constant) folded singleton mass
   SB_CUDA(cudaMemcpyAsync(c->d_part, c->d_base, (size_t)M * 8, cudaMemcpyDeviceToDevice, st));
   A.part_out = c->d_part;
@@ -1517,7 +1441,7 @@ constexpr uint32_t REBALANCE_ITERS = 8;   // measured iterations of the instrume
 
 static int em_rebalance(sb_em_ctx* c) {
   const uint32_t n_warps = c->grid * (EM_THREADS / 32);
-  SB_TRY(dev_alloc(&c->d_dbg, (size_t)n_warps * DBG_SLOTS));
+  SB_TRY(c->res.grow(&c->d_dbg, (size_t)n_warps * DBG_SLOTS));
   SB_CUDA(cudaMemsetAsync(c->d_dbg, 0, (size_t)n_warps * DBG_SLOTS * 8, c->stream));
   const sb_em_params saved = c->params;
   const uint32_t saved_it = c->dbg_it;
@@ -1578,10 +1502,7 @@ extern "C" int sb_flush_l2(sb_em_ctx* c) {
   if (!c) { set_error("null argument"); return SB_ERR_INVALID; }
   SB_CUDA(cudaSetDevice(c->device));
   size_t bytes = std::max<size_t>(c->l2_bytes * 2, (size_t)256 << 20);
-  if (!c->d_flush || c->flush_bytes < bytes) {
-    SB_TRY(dev_alloc((unsigned char**)&c->d_flush, bytes));
-    c->flush_bytes = bytes;
-  }
+  SB_TRY(c->res.grow((unsigned char**)&c->d_flush, bytes));
   SB_CUDA(cudaMemsetAsync(c->d_flush, (int)(c->flush_ctr++ & 0xff), bytes, c->stream));
   SB_CUDA(cudaStreamSynchronize(c->stream));
   return SB_OK;
@@ -1599,6 +1520,12 @@ extern "C" int sb_host_unregister(void* ptr) {
   return SB_OK;
 }
 
+extern "C" int sb_debug_device_memory(uint64_t* out3) {
+  if (!out3) { set_error("null argument"); return SB_ERR_INVALID; }
+  for (int i = 0; i < 3; ++i) out3[i] = g_resource_stats[i].load();
+  return SB_OK;
+}
+
 extern "C" int sb_em_debug_timeline(sb_em_ctx* c, uint64_t* out, uint32_t iteration) {
   if (!c) { set_error("null argument"); return SB_ERR_INVALID; }
   if (!c->prepared) { set_error("not prepared"); return SB_ERR_STATE; }
@@ -1606,7 +1533,7 @@ extern "C" int sb_em_debug_timeline(sb_em_ctx* c, uint64_t* out, uint32_t iterat
   const uint32_t n_warps = c->grid * (EM_THREADS / 32);
   if (!out) {
     // arm: the next sb_em_run records iteration `iteration`
-    SB_TRY(dev_alloc(&c->d_dbg, (size_t)n_warps * DBG_SLOTS));
+    SB_TRY(c->res.grow(&c->d_dbg, (size_t)n_warps * DBG_SLOTS));
     SB_CUDA(cudaMemset(c->d_dbg, 0, (size_t)n_warps * DBG_SLOTS * 8));
     c->dbg_it = iteration;
     c->dbg_enabled = true;

@@ -6,6 +6,7 @@
 #include <vector>
 
 #include "../../include/salmon_b200.h"
+#include "resources.h"
 
 namespace sb {
 
@@ -33,6 +34,8 @@ struct SellDev {
 
 struct sb_em_ctx {
   int device = 0;
+  sb::Resources res;              // every device buffer, the stream and the events below
+  explicit sb_em_ctx(int dev) : device(dev), res(dev) {}
   int n_sm = 0;
   size_t l2_bytes = 0;
   cudaStream_t stream = nullptr;
@@ -149,7 +152,6 @@ struct sb_em_ctx {
 
   // L2 flush
   void* d_flush = nullptr;
-  size_t flush_bytes = 0;
   uint32_t flush_ctr = 0;
 
   // results

@@ -13,6 +13,7 @@
 #include <unistd.h>
 
 #include <algorithm>
+#include <memory>
 #include <parallel/algorithm>
 #include <vector>
 #include <new>
@@ -22,6 +23,7 @@
 #include "map_core.h"
 #include "map_kernels.cuh"
 #include "rescue.cuh"
+#include "resources.h"
 #include "sam_internal.h"
 
 using namespace sbmap;
@@ -61,6 +63,7 @@ struct sb_index {
   uint32_t first_decoy = 0xffffffffu;   // clamped to n_txps by set_meta / build
   // device copies (one device)
   int device = -1;
+  std::unique_ptr<sb::Resources> dev;   // owns them
   uint64_t* d_tx_off = nullptr;
   uint8_t* d_codes = nullptr;
   TableEntry* d_table = nullptr;
@@ -153,12 +156,6 @@ extern "C" sb_index* sb_index_build(uint32_t n_txps, const uint64_t* seq_off, co
 }
 
 extern "C" void sb_index_free(sb_index* ix) {
-  if (!ix) return;
-  if (ix->device >= 0) {
-    cudaSetDevice(ix->device);
-    cudaFree(ix->d_tx_off); cudaFree(ix->d_codes); cudaFree(ix->d_table); cudaFree(ix->d_post);
-    cudaFree(ix->d_packed); cudaFree(ix->d_tx_has_n);
-  }
   delete ix;
 }
 
@@ -342,13 +339,14 @@ extern "C" sb_index* sb_index_load(const char* path) {
 static int upload_big(void* dst, const void* src, size_t bytes) {
   constexpr size_t SL = (size_t)64 << 20;
   if (bytes < 2 * SL) { SB_CUDA(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice)); return SB_OK; }
+  sb::Resources res;   // on the current device
   char* stage[2] = {nullptr, nullptr};
   cudaEvent_t ev[2] = {nullptr, nullptr};
   cudaStream_t st = nullptr;
   int rc = SB_OK;
-  if (cudaMallocHost(&stage[0], SL) != cudaSuccess || cudaMallocHost(&stage[1], SL) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreateWithFlags(&ev[0], cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&ev[1], cudaEventDisableTiming) != cudaSuccess) {
+  if (res.alloc_host(&stage[0], SL) != SB_OK || res.alloc_host(&stage[1], SL) != SB_OK ||
+      res.stream(&st, cudaStreamNonBlocking) != SB_OK ||
+      res.event(&ev[0], cudaEventDisableTiming) != SB_OK || res.event(&ev[1], cudaEventDisableTiming) != SB_OK) {
     cudaGetLastError();
     rc = cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice) == cudaSuccess ? SB_OK : SB_ERR_CUDA;   // plain copy instead
   } else {
@@ -368,11 +366,6 @@ static int upload_big(void* dst, const void* src, size_t bytes) {
     if (cudaStreamSynchronize(st) != cudaSuccess) rc = SB_ERR_CUDA;
   }
   if (rc != SB_OK) sb::set_error("index upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-  if (stage[0]) cudaFreeHost(stage[0]);
-  if (stage[1]) cudaFreeHost(stage[1]);
-  if (ev[0]) cudaEventDestroy(ev[0]);
-  if (ev[1]) cudaEventDestroy(ev[1]);
-  if (st) cudaStreamDestroy(st);
   return rc;
 }
 
@@ -388,18 +381,21 @@ static int index_to_device(sb_index* ix, int device) {
   if (ix->device == device) return SB_OK;
   if (ix->device >= 0) { sb::set_error("index already resident on device %d", ix->device); return SB_ERR_STATE; }
   SB_CUDA(cudaSetDevice(device));
-  SB_CUDA(cudaMalloc(&ix->d_tx_off, ix->tx_off.size() * 8));
-  SB_CUDA(cudaMalloc(&ix->d_codes, std::max<size_t>(ix->codes.size(), 1) + 64));
-  SB_CUDA(cudaMalloc(&ix->d_table, ix->table.size() * sizeof(TableEntry)));
-  SB_CUDA(cudaMalloc(&ix->d_post, std::max<size_t>(ix->post.size(), 1) * sizeof(Posting)));
+  // on any failure `res` releases what was made so far and the index stays host-only, so that a retry starts clean
+  auto res = std::make_unique<sb::Resources>(device);
+  SB_TRY(res->alloc(&ix->d_tx_off, ix->tx_off.size()));
+  SB_TRY(res->alloc(&ix->d_codes, std::max<size_t>(ix->codes.size(), 1) + 64));
+  SB_TRY(res->alloc(&ix->d_table, ix->table.size()));
+  SB_TRY(res->alloc(&ix->d_post, ix->post.size()));
   SB_CUDA(cudaMemcpy(ix->d_tx_off, ix->tx_off.data(), ix->tx_off.size() * 8, cudaMemcpyHostToDevice));
   SB_TRY(upload_big(ix->d_codes, ix->codes.data(), ix->codes.size()));
   SB_TRY(upload_big(ix->d_table, ix->table.data(), ix->table.size() * sizeof(TableEntry)));
   SB_TRY(upload_big(ix->d_post, ix->post.data(), ix->post.size() * sizeof(Posting)));
-  SB_CUDA(cudaMalloc(&ix->d_packed, ix->packed.size() * 8));
-  SB_CUDA(cudaMalloc(&ix->d_tx_has_n, ix->tx_has_n.size()));
+  SB_TRY(res->alloc(&ix->d_packed, ix->packed.size()));
+  SB_TRY(res->alloc(&ix->d_tx_has_n, ix->tx_has_n.size()));
   SB_TRY(upload_big(ix->d_packed, ix->packed.data(), ix->packed.size() * 8));
   SB_CUDA(cudaMemcpy(ix->d_tx_has_n, ix->tx_has_n.data(), ix->tx_has_n.size(), cudaMemcpyHostToDevice));
+  ix->dev = std::move(res);
   ix->device = device;
   return SB_OK;
 }
@@ -950,7 +946,6 @@ __global__ void k_store_records(uint64_t n, const uint64_t* __restrict__ loff, c
 struct Arena {
   uint32_t* labels = nullptr; double* weights = nullptr; uint64_t* counts = nullptr;
   uint64_t *loff = nullptr, *woff = nullptr;        // per store n+1 entries, relative to the store's label / weight base
-  uint64_t cap_l = 0, cap_w = 0, cap_c = 0, cap_o = 0, cap_o_w = 0;   // capacities (entries)
   uint64_t n_l = 0, n_w = 0, n_c = 0, n_o = 0;           // cursors
 };
 struct EqStore {   // a CSR table inside the arena
@@ -964,11 +959,6 @@ struct AggScratch {   // sized for `cap` records
   uint32_t *llen = nullptr, *wlen = nullptr, *idx = nullptr, *idx2 = nullptr, *head = nullptr, *head_scan = nullptr, *first = nullptr;
   void* tmp = nullptr;
   size_t tmp_bytes = 0;
-  void free_all() {
-    void* ps[] = {lstart, wstart, hash, hash2, cls_llen, cls_wlen, llen, wlen, idx, idx2, head, head_scan, first, tmp};
-    for (void* q : ps) cudaFree(q);
-    *this = AggScratch();
-  }
 };
 
 struct FinBufs {   // normalizeAlphas scratch, [M] each
@@ -983,6 +973,8 @@ struct FinBufs {   // normalizeAlphas scratch, [M] each
 
 struct sb_map_ctx {
   int device = 0;
+  sb::Resources res;                 // every buffer, stream and event below (the SAM formatter's are samd's)
+  explicit sb_map_ctx(int dev) : device(dev), res(dev) {}
   int n_sm = 0;
   cudaStream_t stream = nullptr, copy_stream = nullptr;
   sb_index* index = nullptr;
@@ -1061,12 +1053,6 @@ struct sb_map_ctx {
   std::vector<cudaEvent_t> ev_rescue;   // pairs of events around the rescue kernels of each chunk
 };
 
-template <typename T>
-static int dmalloc(T** p, size_t n) {
-  cudaError_t e = cudaMalloc((void**)p, std::max<size_t>(n, 1) * sizeof(T));
-  if (e != cudaSuccess) { sb::set_error("cudaMalloc(%zu) failed: %s", n * sizeof(T), cudaGetErrorString(e)); return SB_ERR_NOMEM; }
-  return SB_OK;
-}
 static inline unsigned nblk(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
 
 // the ungapped shortcut of k_dp_classify is exact only when no cell scores above ma and gaps cost something; under
@@ -1169,20 +1155,22 @@ static double forgetting_mass(std::vector<double>& fm, uint64_t t) {
   return fm[t];
 }
 
-static int agg_reserve(AggScratch& a, uint64_t n) {
+static int agg_reserve(sb_map_ctx* c, uint64_t n) {
+  AggScratch& a = c->agg;
+  sb::Resources& r = c->res;
   if (n <= a.cap) return SB_OK;
-  a.free_all();
+  a.cap = 0;   // until every buffer holds the new size
   const uint64_t cap = std::max<uint64_t>(n, 1024);
-  SB_TRY(dmalloc(&a.lstart, cap)); SB_TRY(dmalloc(&a.wstart, cap)); SB_TRY(dmalloc(&a.hash, cap)); SB_TRY(dmalloc(&a.hash2, cap));
-  SB_TRY(dmalloc(&a.cls_llen, cap + 1)); SB_TRY(dmalloc(&a.cls_wlen, cap + 1));
-  SB_TRY(dmalloc(&a.llen, cap)); SB_TRY(dmalloc(&a.wlen, cap)); SB_TRY(dmalloc(&a.idx, cap)); SB_TRY(dmalloc(&a.idx2, cap));
-  SB_TRY(dmalloc(&a.head, cap + 1)); SB_TRY(dmalloc(&a.head_scan, cap + 1)); SB_TRY(dmalloc(&a.first, cap + 1));
+  SB_TRY(r.grow(&a.lstart, cap)); SB_TRY(r.grow(&a.wstart, cap)); SB_TRY(r.grow(&a.hash, cap)); SB_TRY(r.grow(&a.hash2, cap));
+  SB_TRY(r.grow(&a.cls_llen, cap + 1)); SB_TRY(r.grow(&a.cls_wlen, cap + 1));
+  SB_TRY(r.grow(&a.llen, cap)); SB_TRY(r.grow(&a.wlen, cap)); SB_TRY(r.grow(&a.idx, cap)); SB_TRY(r.grow(&a.idx2, cap));
+  SB_TRY(r.grow(&a.head, cap + 1)); SB_TRY(r.grow(&a.head_scan, cap + 1)); SB_TRY(r.grow(&a.first, cap + 1));
   size_t tb = 0, tb2 = 0, tb3 = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, tb, a.hash, a.hash2, a.idx, a.idx2, (int)cap, 0, 64, (cudaStream_t)0);
   cub::DeviceScan::ExclusiveSum(nullptr, tb2, a.head, a.head_scan, (int)cap + 1, (cudaStream_t)0);
   cub::DeviceScan::ExclusiveSum(nullptr, tb3, a.cls_llen, a.cls_llen, (int)cap + 1, (cudaStream_t)0);
   a.tmp_bytes = std::max(tb, std::max(tb2, tb3));
-  SB_CUDA(cudaMalloc(&a.tmp, a.tmp_bytes));
+  SB_TRY(r.grow((unsigned char**)&a.tmp, a.tmp_bytes));
   a.cap = cap;
   return SB_OK;
 }
@@ -1227,8 +1215,8 @@ extern "C" sb_map_ctx* sb_map_create(sb_index* ix, const sb_map_params* q, int d
     return nullptr;
   }
   if (index_to_device(ix, device) != SB_OK) return nullptr;
-  sb_map_ctx* c = new sb_map_ctx();
-  c->device = device; c->index = ix; c->batch_cap = batch_cap; c->read_len_cap = max_read_len;
+  sb_map_ctx* c = new sb_map_ctx(device);
+  c->index = ix; c->batch_cap = batch_cap; c->read_len_cap = max_read_len;
   Params& p = c->p;
   p.k = q->k; p.stride = q->stride; p.max_occs_per_hit = q->max_occs_per_hit; p.max_read_occ = q->max_read_occ;
   p.max_frag_len = q->max_frag_len; p.band = q->band; p.chain_gap = q->chain_gap; p.range_bins = q->range_bins;
@@ -1250,23 +1238,24 @@ extern "C" sb_map_ctx* sb_map_create(sb_index* ix, const sb_map_params* q, int d
     return nullptr;
   }
   c->fast_ok = fast_dp_exact(p);
-  cudaSetDevice(device);
   cudaDeviceProp prop;
-  cudaGetDeviceProperties(&prop, device);
-  c->n_sm = prop.multiProcessorCount;
-  cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
-  cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking);
-  cudaStreamCreateWithFlags(&c->assign_stream, cudaStreamNonBlocking);
-  for (int s = 0; s < 2; ++s) {
-    cudaEventCreateWithFlags(&c->ev_dp[s], cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&c->ev_asg[s], cudaEventDisableTiming);
+  const cudaError_t de = cudaSetDevice(device);
+  if (de != cudaSuccess || cudaGetDeviceProperties(&prop, device) != cudaSuccess) {
+    sb::set_error("sb_map_create: cannot use device %d: %s", device, cudaGetErrorString(de != cudaSuccess ? de : cudaGetLastError()));
+    delete c;
+    return nullptr;
   }
+  c->n_sm = prop.multiProcessorCount;
   if (const char* e = getenv("SB_MAP_OVERLAP")) c->overlap_assign = atoi(e) ? 1 : 0;
   c->profile = getenv("SB_MAP_PROFILE") ? 1 : 0;
-  cudaEventCreate(&c->ev0); cudaEventCreate(&c->ev1);
+  int rc = SB_OK;
+  auto E = [&](cudaEvent_t* ev, unsigned flags) { if (rc == SB_OK) rc = c->res.event(ev, flags); };
+  auto A = [&](auto** ptr, size_t n) { if (rc == SB_OK) rc = c->res.alloc(ptr, n); };
+  for (cudaStream_t* st : {&c->stream, &c->copy_stream, &c->assign_stream}) if (rc == SB_OK) rc = c->res.stream(st, cudaStreamNonBlocking);
+  E(&c->ev0, cudaEventDefault); E(&c->ev1, cudaEventDefault);
   for (int s = 0; s < 2; ++s) {
-    cudaEventCreateWithFlags(&c->ev_in[s], cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&c->ev_free[s], cudaEventDisableTiming);
+    E(&c->ev_dp[s], cudaEventDisableTiming); E(&c->ev_asg[s], cudaEventDisableTiming);
+    E(&c->ev_in[s], cudaEventDisableTiming); E(&c->ev_free[s], cudaEventDisableTiming);
   }
   const uint32_t cap = p.max_read_occ;
   const size_t B = batch_cap;
@@ -1279,8 +1268,6 @@ extern "C" sb_map_ctx* sb_map_create(sb_index* ix, const sb_map_params* q, int d
   c->seed_blocks = (uint32_t)c->n_sm * 4;
   c->dp_blocks = (uint32_t)c->n_sm * 4;
   BatchBufs& b = c->b;
-  int rc = SB_OK;
-  auto A = [&](auto** ptr, size_t n) { if (rc == SB_OK) rc = dmalloc(ptr, n); };
   // per chunk
   A(&b.n_l, CH); A(&b.n_r, CH); A(&b.cand_l, CH * MAXCAND); A(&b.cand_r, CH * MAXCAND);
   A(&b.score_l, CH * MAXCAND); A(&b.score_r, CH * MAXCAND);
@@ -1308,7 +1295,7 @@ extern "C" sb_map_ctx* sb_map_create(sb_index* ix, const sb_map_params* q, int d
     cub::DeviceRadixSort::SortPairs(nullptr, tb, f.root, f.root2, f.ids, f.memb, (int)M, 0, 32, (cudaStream_t)0);
     cub::DeviceScan::ExclusiveSum(nullptr, tb2, f.head, f.head_scan, (int)M + 1, (cudaStream_t)0);
     f.tmp_bytes = std::max(tb, tb2);
-    if (rc == SB_OK && cudaMalloc(&f.tmp, f.tmp_bytes) != cudaSuccess) rc = SB_ERR_NOMEM;
+    A((unsigned char**)&f.tmp, f.tmp_bytes);
   }
   A(&c->d_overflow, (size_t)c->seed_blocks * SEED_WARPS * MAXSEEDS);
   A(&c->d_next_task, 8); A(&c->d_full_dp, 1);
@@ -1323,32 +1310,33 @@ extern "C" sb_map_ctx* sb_map_create(sb_index* ix, const sb_map_params* q, int d
   std::vector<double>& t = c->init_tables;
   build_fld_host(p, t);
   A(&c->d_fld, (size_t)4 * (p.max_frag_len + 1));
-  if (rc == SB_OK) rc = agg_reserve(c->agg, B);
-  if (rc != SB_OK) { sb_map_destroy(c); return nullptr; }
-  cudaMemcpy(c->d_fld, t.data(), (size_t)4 * c->nf * 8, cudaMemcpyHostToDevice);
-  cudaMemcpy(c->on.hist, t.data() + (size_t)4 * c->nf, (size_t)c->nf * 8, cudaMemcpyHostToDevice);
-  cudaMemcpy(c->on.tot, t.data() + (size_t)5 * c->nf, 8, cudaMemcpyHostToDevice);
-  cudaMemset(c->on.mass_acc, 0, std::max<uint32_t>(c->M, 1) * 8);
-  cudaMemset(c->on.fld_acc, 0, (size_t)c->nf * 8);
-  {
-    const unsigned int mins[2] = {p.max_frag_len, p.max_frag_len};   // FragmentLengthDistribution::min_ starts at max_val
-    cudaMemcpy(c->on.mins, mins, 8, cudaMemcpyHostToDevice);
-  }
-  if (c->M) k_online_init<<<nblk(c->M, 256), 256>>>(c->M, ix->d_tx_off, c->on.mass, c->on.prior, c->on.log_eff);
-  cudaDeviceSynchronize();
-  cudaMemset(c->pr.nmask, 0, 2 * CH * c->pr.mpr * 8);
-  const uint32_t n = p.max_frag_len + 1;
-  c->fld.max_val = p.max_frag_len; c->fld.pmf_live = c->d_fld; c->fld.pmf_cached = c->d_fld + n;
-  c->fld.cmf_cached = c->d_fld + 2 * n; c->fld.cmf_quirk = c->d_fld + 3 * n;
-  cudaMemset(b.ctr, 0, sizeof(Counters));
-  cudaMemset(c->d_full_dp, 0, 8);
   if (p.recover_orphans) {
     RescueBufs& r = c->rb;
     const size_t NT = CH * 2 * MAXCAND;
     A(&r.n_tasks, 1); A(&r.tasks, NT); A(&r.first, CH); A(&r.n_anchor, CH); A(&r.diag, NT); A(&r.score, NT);
     A(&r.pairs, NT); A(&r.n_pairs, CH); A(&r.ctr, 3); A(&c->alt_rs_pairs, NT); A(&c->alt_rs_n_pairs, CH);
-    if (rc != SB_OK) { sb_map_destroy(c); return nullptr; }
   }
+  if (rc == SB_OK) rc = agg_reserve(c, B);
+  if (rc == SB_OK) rc = [&]() -> int {
+    SB_CUDA(cudaMemcpy(c->d_fld, t.data(), (size_t)4 * c->nf * 8, cudaMemcpyHostToDevice));
+    SB_CUDA(cudaMemcpy(c->on.hist, t.data() + (size_t)4 * c->nf, (size_t)c->nf * 8, cudaMemcpyHostToDevice));
+    SB_CUDA(cudaMemcpy(c->on.tot, t.data() + (size_t)5 * c->nf, 8, cudaMemcpyHostToDevice));
+    SB_CUDA(cudaMemset(c->on.mass_acc, 0, std::max<uint32_t>(c->M, 1) * 8));
+    SB_CUDA(cudaMemset(c->on.fld_acc, 0, (size_t)c->nf * 8));
+    const unsigned int mins[2] = {p.max_frag_len, p.max_frag_len};   // FragmentLengthDistribution::min_ starts at max_val
+    SB_CUDA(cudaMemcpy(c->on.mins, mins, 8, cudaMemcpyHostToDevice));
+    if (c->M) k_online_init<<<nblk(c->M, 256), 256>>>(c->M, ix->d_tx_off, c->on.mass, c->on.prior, c->on.log_eff);
+    SB_CUDA(cudaGetLastError());
+    SB_CUDA(cudaDeviceSynchronize());
+    SB_CUDA(cudaMemset(c->pr.nmask, 0, 2 * CH * c->pr.mpr * 8));
+    SB_CUDA(cudaMemset(b.ctr, 0, sizeof(Counters)));
+    SB_CUDA(cudaMemset(c->d_full_dp, 0, 8));
+    return SB_OK;
+  }();
+  if (rc != SB_OK) { sb_map_destroy(c); return nullptr; }
+  const uint32_t n = p.max_frag_len + 1;
+  c->fld.max_val = p.max_frag_len; c->fld.pmf_live = c->d_fld; c->fld.pmf_cached = c->d_fld + n;
+  c->fld.cmf_cached = c->d_fld + 2 * n; c->fld.cmf_quirk = c->d_fld + 3 * n;
   return c;
 }
 
@@ -1356,36 +1344,7 @@ extern "C" void sb_map_destroy(sb_map_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
   cudaDeviceSynchronize();
-  BatchBufs& b = c->b;
-  void* ptrs[] = {b.n_l, b.n_r, b.cand_l, b.cand_r, b.score_l, b.score_r, b.keys, b.n_tasks, b.tasks, b.n_aln, b.tid,
-                  b.score, b.prob, b.pos, b.mate_pos, b.flags, b.flen, b.label, b.weight, b.sc, b.perm_idx, b.perm_tid,
-                  b.bs_tid, b.bs_score, b.bs_idx, b.jh, b.ctr, c->d_in[0][0], c->d_in[0][1], c->d_in[1][0], c->d_in[1][1],
-                  c->d_fld, c->pr.bits, c->pr.nmask, c->d_overflow, c->d_next_task, c->d_full_dp, b.lp,
-                  c->on.mass, c->on.prior, c->on.log_eff, c->on.hist, c->on.tot, c->on.cf, c->on.mass_acc, c->on.fld_acc,
-                  c->on.mins, c->on.fm_rel, c->on.tap_q, c->d_scratch_nf, c->d_list_int, c->d_list_edge, c->d_list_n,
-                  c->d_work, c->d_work2, c->d_ids, c->d_order, c->fin.uniq, c->fin.total, c->fin.hits, c->fin.parent, c->fin.root, c->fin.root2, c->fin.ids, c->fin.memb,
-                  c->fin.head, c->fin.head_scan, c->fin.start, c->fin.proj, c->fin.eff, c->fin.bound, c->fin.tmp};
-  for (void* p : ptrs) cudaFree(p);
-  cudaFree(c->d_dummy_mate);
   sam_dev_destroy(c->samd);
-  {
-    const RescueBufs& r = c->rb;
-    void* rp[] = {r.n_tasks, r.tasks, r.first, r.n_anchor, r.diag, r.score, r.pairs, r.n_pairs, r.ctr, c->alt_rs_pairs,
-                  c->alt_rs_n_pairs};
-    for (void* q : rp) cudaFree(q);
-    for (cudaEvent_t e : c->ev_rescue) cudaEventDestroy(e);
-  }
-  cudaFree(c->alt_n_l); cudaFree(c->alt_n_r); cudaFree(c->alt_cand_l); cudaFree(c->alt_cand_r); cudaFree(c->alt_score_l); cudaFree(c->alt_score_r);
-  for (int s = 0; s < 2; ++s) { if (c->ev_dp[s]) cudaEventDestroy(c->ev_dp[s]); if (c->ev_asg[s]) cudaEventDestroy(c->ev_asg[s]); }
-  if (c->assign_stream) cudaStreamDestroy(c->assign_stream);
-  c->agg.free_all();
-  cudaFree(c->arena.labels); cudaFree(c->arena.weights); cudaFree(c->arena.counts); cudaFree(c->arena.loff); cudaFree(c->arena.woff);
-  for (cudaEvent_t e : c->ev_seed) cudaEventDestroy(e);
-  if (c->ev0) cudaEventDestroy(c->ev0);
-  if (c->ev1) cudaEventDestroy(c->ev1);
-  for (int s = 0; s < 2; ++s) { if (c->ev_in[s]) cudaEventDestroy(c->ev_in[s]); if (c->ev_free[s]) cudaEventDestroy(c->ev_free[s]); }
-  if (c->stream) cudaStreamDestroy(c->stream);
-  if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
   delete c;
 }
 
@@ -1402,7 +1361,8 @@ extern "C" int sb_map_set_option(sb_map_ctx* c, const char* key, int64_t value) 
   if (!strcmp(key, "ascii_reads")) {
     if (value && c->variant == 0) { sb::set_error("ascii_reads needs the warp kernels (variant 1)"); return SB_ERR_INVALID; }
     c->ascii = value ? 1 : 0;
-    if (c->d_dummy_mate) { cudaFree(c->d_dummy_mate); c->d_dummy_mate = nullptr; }   // its N codes depend on the encoding
+    c->res.release(c->d_dummy_mate);   // its N codes depend on the encoding
+    c->d_dummy_mate = nullptr;
     return SB_OK;
   }
   if (!strcmp(key, "overlap_assign")) { c->overlap_assign = value ? 1 : 0; return SB_OK; }
@@ -1429,19 +1389,6 @@ extern "C" int sb_map_set_option(sb_map_ctx* c, const char* key, int64_t value) 
   return SB_ERR_INVALID;
 }
 
-template <typename T>
-static int arena_grow(T** p, uint64_t* cap, uint64_t used, uint64_t need, cudaStream_t st) {
-  if (need <= *cap) return SB_OK;
-  uint64_t ncap = std::max<uint64_t>(need, *cap * 2);
-  T* q = nullptr;
-  SB_TRY(dmalloc(&q, ncap));
-  if (used) SB_CUDA(cudaMemcpyAsync(q, *p, used * sizeof(T), cudaMemcpyDeviceToDevice, st));
-  SB_CUDA(cudaStreamSynchronize(st));
-  cudaFree(*p);
-  *p = q; *cap = ncap;
-  return SB_OK;
-}
-
 // records -> classes (per batch over the read slots, and at finish over all batch classes); the table is appended to
 // the arena
 static int aggregate(sb_map_ctx* c, Records R, EqStore& out) {
@@ -1464,15 +1411,13 @@ static int aggregate(sb_map_ctx* c, Records R, EqStore& out) {
   k_class_sizes<<<nblk(n, 256), 256, 0, st>>>(R, a.head, a.head_scan, a.idx2, a.first, a.cls_llen, a.cls_wlen);
   out.base_o = ar.n_o; out.base_c = ar.n_c;
   {
-    // R may point into the arena (finish): growing moves it, so remember the offsets of its arrays
-    const bool in_arena = R.labels >= ar.labels && R.labels < ar.labels + ar.cap_l;
+    // R may be the arena's own tables (finish): growing moves them, so remember the offsets of its arrays
+    const bool in_arena = R.labels && R.labels == ar.labels;
     const uint64_t ro_l = in_arena ? (uint64_t)(R.labels - ar.labels) : 0, ro_w = in_arena ? (uint64_t)(R.weights - ar.weights) : 0,
                    ro_c = (in_arena && R.counts) ? (uint64_t)(R.counts - ar.counts) : 0;
-    SB_TRY(arena_grow(&ar.loff, &ar.cap_o, ar.n_o, ar.n_o + nc + 1, st));
-    uint64_t capw = ar.cap_o_w;
-    SB_TRY(arena_grow(&ar.woff, &capw, ar.n_o, ar.n_o + nc + 1, st));
-    ar.cap_o_w = capw;
-    SB_TRY(arena_grow(&ar.counts, &ar.cap_c, ar.n_c, ar.n_c + nc, st));
+    SB_TRY(c->res.grow_keep(&ar.loff, ar.n_o, ar.n_o + nc + 1, st));
+    SB_TRY(c->res.grow_keep(&ar.woff, ar.n_o, ar.n_o + nc + 1, st));
+    SB_TRY(c->res.grow_keep(&ar.counts, ar.n_c, ar.n_c + nc, st));
     t = a.tmp_bytes;
     SB_CUDA(cub::DeviceScan::ExclusiveSum(a.tmp, t, a.cls_llen, ar.loff + out.base_o, (int)nc + 1, st));
     t = a.tmp_bytes;
@@ -1482,8 +1427,8 @@ static int aggregate(sb_map_ctx* c, Records R, EqStore& out) {
     SB_CUDA(cudaMemcpyAsync(&tw, ar.woff + out.base_o + nc, 8, cudaMemcpyDeviceToHost, st));
     SB_CUDA(cudaStreamSynchronize(st));
     out.base_l = ar.n_l; out.base_w = ar.n_w;
-    SB_TRY(arena_grow(&ar.labels, &ar.cap_l, ar.n_l, ar.n_l + tl, st));
-    SB_TRY(arena_grow(&ar.weights, &ar.cap_w, ar.n_w, ar.n_w + tw, st));
+    SB_TRY(c->res.grow_keep(&ar.labels, ar.n_l, ar.n_l + tl, st));
+    SB_TRY(c->res.grow_keep(&ar.weights, ar.n_w, ar.n_w + tw, st));
     if (in_arena) { R.labels = ar.labels + ro_l; R.weights = ar.weights + ro_w; if (R.counts) R.counts = ar.counts + ro_c; }
     k_class_reduce<<<nblk((uint64_t)nc * 32, 256), 256, 0, st>>>(R, nc, a.first, a.idx2, ar.loff + out.base_o,
                                                                 ar.woff + out.base_o, ar.labels + out.base_l,
@@ -1514,7 +1459,7 @@ static int map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, u
     // second mate: a device buffer of N codes -- no k-mer, no seed, no candidate -- so every mapping is a left "orphan",
     // which is exactly how the auxiliary model treats a single-end read (getAmbigFragLengthProb, :642-650 / :2186-2200)
     if (!c->d_dummy_mate) {
-      SB_CUDA(cudaMalloc(&c->d_dummy_mate, (size_t)c->batch_cap * c->read_len_cap));
+      SB_TRY(c->res.alloc(&c->d_dummy_mate, (size_t)c->batch_cap * c->read_len_cap));
       SB_CUDA(cudaMemset(c->d_dummy_mate, c->ascii ? 'N' : 4, (size_t)c->batch_cap * c->read_len_cap));
     }
   }
@@ -1592,7 +1537,7 @@ static int map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, u
       DpIo io{bc.n_tasks, bc.tasks, bc.cand_l, bc.cand_r, bc.score_l, bc.score_r, c->d_next_task, c->d_next_task + 4,
               c->d_list_int, c->d_list_edge, c->d_list_n, c->d_full_dp};
       const uint32_t npos = (L - p.k) / p.stride + 1 + (((L - p.k) % p.stride) ? 1u : 0u);   // seed positions per mate
-      while (c->ev_seed.size() < 2 * (size_t)(ch + 1)) { cudaEvent_t e; cudaEventCreate(&e); c->ev_seed.push_back(e); }
+      while (c->ev_seed.size() < 2 * (size_t)(ch + 1)) { cudaEvent_t e; SB_TRY(c->res.event(&e, cudaEventDefault)); c->ev_seed.push_back(e); }
       SB_CUDA(cudaEventRecord(c->ev_seed[2 * ch], st));
       if (c->read_len_cap <= 128) {
         if (npos <= 32) k_seed_chain_w<2, 1><<<c->seed_blocks, SeedCfg<2>::WARPS * 32, 0, st>>>(ix, p, c->pr, cn, L, so);
@@ -1620,7 +1565,7 @@ static int map_batch(sb_map_ctx* c, const uint8_t* left, const uint8_t* right, u
     RescueBufs rb = c->rb;
     if (resc) {
       if (ovl && set) { rb.pairs = c->alt_rs_pairs; rb.n_pairs = c->alt_rs_n_pairs; }
-      while (c->ev_rescue.size() < 2 * (size_t)(ch + 1)) { cudaEvent_t e; cudaEventCreate(&e); c->ev_rescue.push_back(e); }
+      while (c->ev_rescue.size() < 2 * (size_t)(ch + 1)) { cudaEvent_t e; SB_TRY(c->res.event(&e, cudaEventDefault)); c->ev_rescue.push_back(e); }
       SB_CUDA(cudaEventRecord(c->ev_rescue[2 * ch], st));
       SB_CUDA(cudaMemsetAsync(rb.n_tasks, 0, 4, st));
       k_rescue_select<<<nblk(cn, 128), 128, 0, st>>>(p, cn, L, bc.n_l, bc.n_r, bc.cand_l, bc.cand_r, bc.score_l, bc.score_r, rb);
@@ -1824,8 +1769,9 @@ extern "C" int sb_rescue_search_tap(int device, uint32_t n, const uint8_t* pats,
   uint8_t *d_p = nullptr, *d_w = nullptr, *d_hn = nullptr;
   uint64_t *d_po = nullptr, *d_wo = nullptr, *d_pk = nullptr;
   int32_t *d_k = nullptr, *d_d = nullptr, *d_e = nullptr;
+  sb::Resources res;   // on the current device
   int rc = SB_OK;
-  auto A = [&](auto** ptr, size_t m) { if (rc == SB_OK) rc = dmalloc(ptr, m); };
+  auto A = [&](auto** ptr, size_t m) { if (rc == SB_OK) rc = res.alloc(ptr, m); };
   A(&d_p, np); A(&d_w, nw); A(&d_hn, n); A(&d_po, n + 1); A(&d_wo, n + 1); A(&d_pk, packed.size()); A(&d_k, n);
   A(&d_d, n); A(&d_e, n);
   cudaError_t e = cudaSuccess;
@@ -1845,8 +1791,6 @@ extern "C" int sb_rescue_search_tap(int device, uint32_t n, const uint8_t* pats,
     if (e == cudaSuccess) e = cudaMemcpy(dist, d_d, (size_t)n * 4, cudaMemcpyDeviceToHost);
     if (e == cudaSuccess) e = cudaMemcpy(end, d_e, (size_t)n * 4, cudaMemcpyDeviceToHost);
   }
-  void* ptrs[] = {d_p, d_w, d_hn, d_po, d_wo, d_pk, d_k, d_d, d_e};
-  for (void* q : ptrs) cudaFree(q);
   if (rc != SB_OK) return rc;
   if (e != cudaSuccess) { sb::set_error("sb_rescue_search_tap: %s", cudaGetErrorString(e)); return SB_ERR_CUDA; }
   return SB_OK;
@@ -1955,7 +1899,7 @@ extern "C" int sb_map_finish(sb_map_ctx* c, sb_map_result* out) {
   Arena& ar = c->arena;
   const uint64_t mark_l = ar.n_l, mark_w = ar.n_w, mark_c = ar.n_c, mark_o = ar.n_o;   // the merged table is temporary
   if (n) {
-    SB_TRY(agg_reserve(c->agg, n));
+    SB_TRY(agg_reserve(c, n));
     AggScratch& a = c->agg;
     uint64_t i = 0;
     for (auto& s : c->stores) {   // the batch tables are the records: label / weight starts are arena positions
@@ -2163,8 +2107,7 @@ struct sb_eq_builder {
   sb_map_ctx* c = nullptr;          // only stream, aggregation scratch and arena are used
   uint32_t n_txps = 0;
   uint64_t n_groups = 0;
-  // device staging of one batch
-  uint64_t cap_n = 0, cap_l = 0, cap_w = 0;
+  // device staging of one batch (owned by c)
   uint64_t *d_loff = nullptr, *d_woff = nullptr, *d_counts = nullptr;
   uint32_t* d_labels = nullptr;
   double* d_weights = nullptr;
@@ -2180,17 +2123,14 @@ extern "C" sb_eq_builder* sb_eq_create(uint32_t n_txps, int device) {
   if (device < 0 || device >= n_dev) { sb::set_error("device %d out of range", device); return nullptr; }
   if (cudaSetDevice(device) != cudaSuccess) { sb::set_error("cudaSetDevice failed"); return nullptr; }
   sb_eq_builder* b = new sb_eq_builder();
-  b->c = new sb_map_ctx();
-  b->c->device = device;
+  b->c = new sb_map_ctx(device);
   b->n_txps = n_txps;
-  if (cudaStreamCreate(&b->c->stream) != cudaSuccess) { sb::set_error("cudaStreamCreate failed"); delete b->c; delete b; return nullptr; }
+  if (b->c->res.stream(&b->c->stream, cudaStreamDefault) != SB_OK) { delete b->c; delete b; return nullptr; }
   return b;
 }
 
 extern "C" void sb_eq_destroy(sb_eq_builder* b) {
   if (!b) return;
-  cudaSetDevice(b->c->device);
-  cudaFree(b->d_loff); cudaFree(b->d_woff); cudaFree(b->d_counts); cudaFree(b->d_labels); cudaFree(b->d_weights);
   sb_map_destroy(b->c);
   delete b;
 }
@@ -2203,16 +2143,6 @@ __global__ void k_eq_records(uint32_t n, const uint64_t* __restrict__ loff, cons
   if (i >= n) return;
   lstart[i] = loff[i]; llen[i] = (uint32_t)(loff[i + 1] - loff[i]);
   wstart[i] = woff[i]; wlen[i] = (uint32_t)(woff[i + 1] - woff[i]);
-}
-template <typename T>
-int regrow(T** p, uint64_t* cap, uint64_t need) {
-  if (need <= *cap) return SB_OK;
-  cudaFree(*p);
-  *p = nullptr;
-  const uint64_t c = std::max<uint64_t>(need + need / 2, 1024);
-  SB_CUDA(cudaMalloc(p, c * sizeof(T)));
-  *cap = c;
-  return SB_OK;
 }
 }  // namespace
 
@@ -2236,18 +2166,16 @@ extern "C" int sb_eq_add_batch(sb_eq_builder* b, uint32_t n, const uint64_t* lab
   sb_map_ctx* c = b->c;
   SB_CUDA(cudaSetDevice(c->device));
   cudaStream_t st = c->stream;
-  uint64_t cn = b->cap_n, cn2 = b->cap_n, cn3 = b->cap_n;
-  SB_TRY(regrow(&b->d_loff, &cn, (uint64_t)n + 1)); SB_TRY(regrow(&b->d_woff, &cn2, (uint64_t)n + 1));
-  SB_TRY(regrow(&b->d_counts, &cn3, (uint64_t)n + 1));
-  b->cap_n = std::min(cn, std::min(cn2, cn3));
-  SB_TRY(regrow(&b->d_labels, &b->cap_l, nl));
-  SB_TRY(regrow(&b->d_weights, &b->cap_w, nw));
+  SB_TRY(c->res.grow(&b->d_loff, (size_t)n + 1)); SB_TRY(c->res.grow(&b->d_woff, (size_t)n + 1));
+  SB_TRY(c->res.grow(&b->d_counts, (size_t)n + 1));
+  SB_TRY(c->res.grow(&b->d_labels, nl));
+  SB_TRY(c->res.grow(&b->d_weights, nw));
   SB_CUDA(cudaMemcpyAsync(b->d_loff, label_off, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, st));
   SB_CUDA(cudaMemcpyAsync(b->d_woff, weight_off, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, st));
   SB_CUDA(cudaMemcpyAsync(b->d_labels, labels, nl * 4, cudaMemcpyHostToDevice, st));
   SB_CUDA(cudaMemcpyAsync(b->d_weights, weights, nw * 8, cudaMemcpyHostToDevice, st));
   if (counts) SB_CUDA(cudaMemcpyAsync(b->d_counts, counts, (size_t)n * 8, cudaMemcpyHostToDevice, st));
-  SB_TRY(agg_reserve(c->agg, n));
+  SB_TRY(agg_reserve(c, n));
   AggScratch& a = c->agg;
   k_eq_records<<<nblk(n, 256), 256, 0, st>>>(n, b->d_loff, b->d_woff, a.lstart, a.llen, a.wstart, a.wlen);
   Records R{n, a.lstart, a.llen, a.wstart, a.wlen, b->d_labels, b->d_weights, counts ? b->d_counts : nullptr};
@@ -2281,7 +2209,7 @@ extern "C" int sb_eq_finish(sb_eq_builder* b, sb_eq_table* out) {
   Arena& ar = c->arena;
   const uint64_t mark_l = ar.n_l, mark_w = ar.n_w, mark_c = ar.n_c, mark_o = ar.n_o;
   if (n) {
-    SB_TRY(agg_reserve(c->agg, n));
+    SB_TRY(agg_reserve(c, n));
     AggScratch& a = c->agg;
     uint64_t i = 0;
     for (auto& s : c->stores) {

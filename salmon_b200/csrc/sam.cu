@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "sam_core.h"
+#include "resources.h"
 #include "sam_internal.h"
 
 using namespace sbsam;
@@ -189,33 +190,22 @@ __global__ void __launch_bounds__(256) k_sam_write(SamArgs A, uint32_t f0, uint3
   }
 }
 
-template <typename T>
-int dgrow(T** p, size_t* cap, size_t need) {
-  if (need <= *cap) return SB_OK;
-  cudaFree(*p);
-  *p = nullptr;
-  *cap = 0;
-  const size_t n = std::max<size_t>(need, 1);
-  SB_CUDA(cudaMalloc((void**)p, n * sizeof(T)));
-  *cap = n;
-  return SB_OK;
-}
-
 }  // namespace
 
 struct SamDev {
+  sb::Resources res;              // every buffer and event below, made and released on the mapping context's device
   sb_sam* s = nullptr;
   uint32_t B = 0, Lcap = 0, cap = 0;
   sbmap::SamSide side{};
   uint8_t* codes[2] = {nullptr, nullptr};
   uint8_t* qual[2] = {nullptr, nullptr};
-  char* names = nullptr; size_t names_cap = 0;
+  char* names = nullptr;
   uint64_t* name_off = nullptr;
   uint64_t *sam_bytes = nullptr, *sam_off = nullptr, *un_bytes = nullptr, *un_off = nullptr;
   uint64_t* h_off = nullptr;     // page-locked copy of sam_off
   unsigned long long* records = nullptr;   // [0]: records of the batch (device), [1]: its page-locked copy
-  char* win = nullptr; size_t win_cap = 0;
-  char* un = nullptr; size_t un_cap = 0;
+  char* win = nullptr;
+  char* un = nullptr;
   uint32_t* ref_len = nullptr; uint64_t* rname_off = nullptr; char* rnames = nullptr;
   void* tmp = nullptr; size_t tmp_bytes = 0;
   cudaEvent_t ev[2] = {nullptr, nullptr};
@@ -226,41 +216,33 @@ int sam_dev_create(SamDev** out, sb_sam* s, uint32_t B, uint32_t Lcap, uint32_t 
   *out = d;
   d->s = s; d->B = B; d->Lcap = Lcap; d->cap = cap;
   const size_t BC = (size_t)B * cap;
-  SB_CUDA(cudaMalloc(&d->side.n_out, (size_t)B * 4));
-  SB_CUDA(cudaMalloc(&d->side.decoy, B));
-  SB_CUDA(cudaMalloc(&d->side.score1, BC * 4));
-  SB_CUDA(cudaMalloc(&d->side.score2, BC * 4));
-  for (int m = 0; m < 2; ++m) SB_CUDA(cudaMalloc(&d->codes[m], (size_t)B * Lcap));
+  sb::Resources& r = d->res;
+  SB_TRY(r.alloc(&d->side.n_out, B));
+  SB_TRY(r.alloc(&d->side.decoy, B));
+  SB_TRY(r.alloc(&d->side.score1, BC));
+  SB_TRY(r.alloc(&d->side.score2, BC));
+  for (int m = 0; m < 2; ++m) SB_TRY(r.alloc(&d->codes[m], (size_t)B * Lcap));
   if (s->flags & SB_SAM_QUALITIES)
-    for (int m = 0; m < 2; ++m) SB_CUDA(cudaMalloc(&d->qual[m], (size_t)B * Lcap));
-  SB_CUDA(cudaMalloc(&d->name_off, ((size_t)B + 1) * 8));
-  SB_CUDA(cudaMalloc(&d->sam_bytes, ((size_t)B + 1) * 8)); SB_CUDA(cudaMalloc(&d->sam_off, ((size_t)B + 1) * 8));
-  SB_CUDA(cudaMalloc(&d->un_bytes, ((size_t)B + 1) * 8)); SB_CUDA(cudaMalloc(&d->un_off, ((size_t)B + 1) * 8));
-  SB_CUDA(cudaMallocHost(&d->h_off, ((size_t)B + 2) * 8));
-  SB_CUDA(cudaMalloc(&d->records, 8));
+    for (int m = 0; m < 2; ++m) SB_TRY(r.alloc(&d->qual[m], (size_t)B * Lcap));
+  SB_TRY(r.alloc(&d->name_off, (size_t)B + 1));
+  SB_TRY(r.alloc(&d->sam_bytes, (size_t)B + 1)); SB_TRY(r.alloc(&d->sam_off, (size_t)B + 1));
+  SB_TRY(r.alloc(&d->un_bytes, (size_t)B + 1)); SB_TRY(r.alloc(&d->un_off, (size_t)B + 1));
+  SB_TRY(r.alloc_host(&d->h_off, (size_t)B + 2));
+  SB_TRY(r.alloc(&d->records, 1));
   const uint32_t M = s->n_txps;
-  SB_CUDA(cudaMalloc(&d->ref_len, std::max<size_t>(M, 1) * 4));
-  SB_CUDA(cudaMalloc(&d->rname_off, ((size_t)M + 1) * 8));
-  SB_CUDA(cudaMalloc(&d->rnames, std::max<size_t>(s->rnames.size(), 1)));
+  SB_TRY(r.alloc(&d->ref_len, M));
+  SB_TRY(r.alloc(&d->rname_off, (size_t)M + 1));
+  SB_TRY(r.alloc(&d->rnames, s->rnames.size()));
   SB_CUDA(cudaMemcpy(d->ref_len, s->ref_len.data(), (size_t)M * 4, cudaMemcpyHostToDevice));
   SB_CUDA(cudaMemcpy(d->rname_off, s->rname_off.data(), ((size_t)M + 1) * 8, cudaMemcpyHostToDevice));
   SB_CUDA(cudaMemcpy(d->rnames, s->rnames.data(), s->rnames.size(), cudaMemcpyHostToDevice));
   SB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, d->tmp_bytes, d->sam_bytes, d->sam_off, (int)B + 1));
-  SB_CUDA(cudaMalloc(&d->tmp, d->tmp_bytes));
-  for (int i = 0; i < 2; ++i) SB_CUDA(cudaEventCreate(&d->ev[i]));
+  SB_TRY(r.alloc((unsigned char**)&d->tmp, d->tmp_bytes));
+  for (int i = 0; i < 2; ++i) SB_TRY(r.event(&d->ev[i], cudaEventDefault));
   return SB_OK;
 }
 
-void sam_dev_destroy(SamDev* d) {
-  if (!d) return;
-  void* ps[] = {d->side.n_out, d->side.decoy, d->side.score1, d->side.score2, d->codes[0], d->codes[1], d->qual[0],
-                d->qual[1], d->names, d->name_off, d->sam_bytes, d->sam_off, d->un_bytes, d->un_off, d->win, d->un,
-                d->ref_len, d->rname_off, d->rnames, d->tmp, d->records};
-  for (void* p : ps) cudaFree(p);
-  if (d->h_off) cudaFreeHost(d->h_off);
-  for (int i = 0; i < 2; ++i) if (d->ev[i]) cudaEventDestroy(d->ev[i]);
-  delete d;
-}
+void sam_dev_destroy(SamDev* d) { delete d; }
 
 sbmap::SamSide sam_dev_side(SamDev* d) { return d->side; }
 
@@ -281,7 +263,7 @@ int sam_dev_format(SamDev* d, cudaStream_t st, const SamBatch& b, const uint8_t*
     if (b.paired) SB_CUDA(cudaMemcpyAsync(d->qual[1], qr, (size_t)n * L, cudaMemcpyHostToDevice, st));
   }
   const uint64_t name_bytes = name_off[n] - name_off[0];
-  SB_TRY(dgrow(&d->names, &d->names_cap, name_bytes));
+  SB_TRY(d->res.grow(&d->names, name_bytes));
   SB_CUDA(cudaMemcpyAsync(d->names, names + name_off[0], name_bytes, cudaMemcpyHostToDevice, st));
   SB_CUDA(cudaMemcpyAsync(d->name_off, name_off, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, st));
   SamArgs A;
@@ -310,7 +292,7 @@ int sam_dev_format(SamDev* d, cudaStream_t st, const SamBatch& b, const uint8_t*
   const uint64_t n_records = d->h_off[n + 1];
   SB_CUDA(cudaEventElapsedTime(&ms, d->ev[0], d->ev[1]));
   *format_ms += ms;
-  SB_TRY(dgrow(&d->un, &d->un_cap, un_total));
+  SB_TRY(d->res.grow(&d->un, un_total));
   // windows of whole fragments that fit the device buffer (a fragment larger than the buffer gets a window of its own,
   // and the buffer grows to hold it)
   const uint64_t W = std::max<uint64_t>(window_bytes, 1);
@@ -324,15 +306,15 @@ int sam_dev_format(SamDev* d, cudaStream_t st, const SamBatch& b, const uint8_t*
       }
       f1 = lo;
     }
-    const uint64_t bytes = d->h_off[f1] - d->h_off[f0];
-    SB_TRY(dgrow(&d->win, &d->win_cap, std::max<uint64_t>(bytes, std::min<uint64_t>(W, d->h_off[n]))));
+    const uint64_t bytes = d->h_off[f1] - d->h_off[f0], want = std::max<uint64_t>(bytes, std::min<uint64_t>(W, d->h_off[n]));
+    SB_TRY(d->res.grow(&d->win, want));
     SB_CUDA(cudaEventRecord(d->ev[0], st));
     const uint32_t warps = f1 - f0, blocks = std::min<uint32_t>((warps + 7) / 8, 65535u);
     k_sam_write<<<blocks, 256, 0, st>>>(A, f0, f1, d->sam_off, d->un_off, d->win, d->un);
     SB_CUDA(cudaEventRecord(d->ev[1], st));
     if (bytes) {
       const double t0 = now_ms();
-      const int slot = take_slot(s, std::max<uint64_t>(bytes, d->win_cap));
+      const int slot = take_slot(s, want);
       if (slot < 0) return SB_ERR_NOMEM;
       const double t1 = now_ms();
       SB_CUDA(cudaMemcpyAsync(s->pin[slot], d->win, bytes, cudaMemcpyDeviceToHost, st));

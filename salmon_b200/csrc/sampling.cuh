@@ -253,7 +253,7 @@ __global__ void k_gibbs_out(uint32_t M, const double* __restrict__ mu, const dou
 static int build_cdf(sb_em_ctx* c, const uint8_t* valid, int mode, uint64_t* total_out) {
   cudaStream_t st = c->stream;
   const uint64_t C = c->C;
-  SB_TRY(dev_alloc(&c->d_cdf, C + 1));
+  SB_TRY(c->res.grow(&c->d_cdf, C + 1));
   if (C) {
     k_cdf_weights<<<nblk(C, 256), 256, 0, st>>>(C, c->d_off, c->d_counts, valid, mode, c->d_packed);
     size_t tb = c->tmp_bytes;
@@ -275,14 +275,14 @@ extern "C" int sb_bootstrap(sb_em_ctx* c, const sb_em_params* p, double num_mapp
   cudaStream_t st = c->stream;
   const uint64_t C = c->C;
   const uint32_t M = c->M, R = c->n_rows, Cm = c->n_cls;
-  SB_TRY(dev_alloc(&c->d_active, (size_t)M));
-  SB_TRY(dev_alloc(&c->d_valid_boot, C));
-  SB_TRY(dev_alloc(&c->d_samp, (size_t)Cm + M + 1));
-  SB_TRY(dev_alloc(&c->ov_cnt, (size_t)Cm + 1));
-  SB_TRY(dev_alloc(&c->ov_base_tid, (size_t)M));
-  SB_TRY(dev_alloc(&c->ov_base_row, (size_t)R + 1));
-  SB_TRY(dev_alloc(&c->ov_alpha0_row, (size_t)R + 1));
-  SB_TRY(dev_alloc(&c->ov_alpha0_tid, (size_t)M));
+  SB_TRY(c->res.grow(&c->d_active, (size_t)M));
+  SB_TRY(c->res.grow(&c->d_valid_boot, C));
+  SB_TRY(c->res.grow(&c->d_samp, (size_t)Cm + M + 1));
+  SB_TRY(c->res.grow(&c->ov_cnt, (size_t)Cm + 1));
+  SB_TRY(c->res.grow(&c->ov_base_tid, (size_t)M));
+  SB_TRY(c->res.grow(&c->ov_base_row, (size_t)R + 1));
+  SB_TRY(c->res.grow(&c->ov_alpha0_row, (size_t)R + 1));
+  SB_TRY(c->res.grow(&c->ov_alpha0_tid, (size_t)M));
   // active transcripts: members of ANY class (:582-590)
   SB_CUDA(cudaMemsetAsync(c->d_active, 0, M, st));
   unsigned long long* d_nact = (unsigned long long*)(c->d_scalars + 40);
@@ -368,11 +368,11 @@ extern "C" int sb_gibbs(sb_em_ctx* c, const double* alphas_init, int use_vbem, i
   const int perTxp = use_vbem ? per_txp_prior : 1;
   double prior = 1e-3;
   if (use_vbem) prior = perTxp ? (vb_prior < 1.0 ? 1.0 : vb_prior) : (vb_prior < 1e-3 ? 1e-3 : vb_prior);
-  SB_TRY(dev_alloc(&c->d_active, (size_t)M));
-  SB_TRY(dev_alloc(&c->d_gibbs_cnt, (size_t)M));
-  SB_TRY(dev_alloc(&c->d_gibbs_mu, (size_t)M));
-  SB_TRY(dev_alloc(&c->d_gibbs_prior, (size_t)M));
-  SB_TRY(dev_alloc(&c->d_gibbs_out, (size_t)2 * M));   // [init | out]
+  SB_TRY(c->res.grow(&c->d_active, (size_t)M));
+  SB_TRY(c->res.grow(&c->d_gibbs_cnt, (size_t)M));
+  SB_TRY(c->res.grow(&c->d_gibbs_mu, (size_t)M));
+  SB_TRY(c->res.grow(&c->d_gibbs_prior, (size_t)M));
+  SB_TRY(c->res.grow(&c->d_gibbs_out, (size_t)2 * M));   // [init | out]
   double* d_init = c->d_gibbs_out;
   double* d_out = c->d_gibbs_out + M;
   SB_CUDA(cudaMemcpyAsync(d_init, alphas_init, (size_t)M * 8, cudaMemcpyHostToDevice, st));

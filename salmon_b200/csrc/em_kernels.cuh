@@ -607,16 +607,23 @@ __device__ __forceinline__ double sum_partials(const double* part, uint32_t n, d
 
 // lagged logNorm: alphaSum of THIS iteration's input = the per-block partials written by
 // the previous P2 (complete since the last grid barrier / kernel boundary).  Any common
-// factor in theta cancels in P1/P2 (DESIGN.md).  Warp 0 only; result in scratch[33].
-__device__ __forceinline__ void lag_lognorm_warp0(const EmArgs& A, uint32_t par, uint32_t nblk,
-                                                  double* scratch) {
-  if (threadIdx.x < 32) {
-    const double* part = A.sum_partial + (size_t)(par ^ 1u) * nblk;
-    long long acc = 0;
-    for (uint32_t i = threadIdx.x; i < nblk; i += 32) acc += __double_as_longlong(__ldcg(&part[i]));
-    acc = warp_sum_ll(acc);
-    if (threadIdx.x == 0) scratch[33] = digamma_pos((double)acc / A.sum_scale + A.inactive_sum);
-  }
+// factor in theta cancels in P1/P2 (DESIGN.md).  One whole warp; result in scratch[33].
+__device__ __forceinline__ void lag_lognorm_warp(const EmArgs& A, uint32_t par, uint32_t nblk, double* scratch) {
+  const uint32_t lane = threadIdx.x & 31u;
+  const double* part = A.sum_partial + (size_t)(par ^ 1u) * nblk;
+  long long acc = 0;
+  for (uint32_t i = lane; i < nblk; i += 32) acc += __double_as_longlong(__ldcg(&part[i]));
+  acc = warp_sum_ll(acc);
+  if (lane == 0) scratch[33] = digamma_pos((double)acc / A.sum_scale + A.inactive_sum);
+}
+// Persistent kernel: the first warp of the block to finish its P1 home range computes the lagged logNorm (claim in
+// scratch[34], cleared after the grid barrier that follows P1).  That warp has time to spare before the barrier,
+// while a fixed warp that did it before its home range started P1 about 2.5 us after the others.
+__device__ __forceinline__ void lag_lognorm_first_warp(const EmArgs& A, uint32_t par, uint32_t nblk,
+                                                       double* scratch) {
+  uint32_t first = 0;
+  if ((threadIdx.x & 31u) == 0) first = atomicAdd(reinterpret_cast<unsigned int*>(&scratch[34]), 1u) == 0u;
+  if (__shfl_sync(0xffffffffu, first, 0)) lag_lognorm_warp(A, par, nblk, scratch);
 }
 
 __device__ __forceinline__ void p2_finish(const EmArgs& A, double* scratch, P2Acc& pa,
@@ -664,19 +671,23 @@ __global__ void __launch_bounds__(EM_THREADS, EM_MIN_BLOCKS) k_em_persistent(con
     const uint32_t par = it & 1u;
     const bool dbg_acc = A.dbg && A.dbg_it == DBG_ACCUMULATE && it > 0;
     if (bid == 0 && threadIdx.x == 0) A.maxrel[par] = 0ull;
-    if (VBEM && it > 0) lag_lognorm_warp0(A, par, nblk, scratch);  // consumed after the next barrier
     P2Acc pa{0ll, 0.0};
     SB_DBG(0)
     SB_ACC_BEGIN(t1, 3)
     W.dbg = (A.dbg && it == A.dbg_it) ? &A.dbg[(size_t)gwarp * DBG_SLOTS] : nullptr;
-    // P2's home stream lands while this warp takes queue items and during the grid barrier
-    run_phase<1, VBEM, true>(A, W, R1, bid, nblk, 0.0, 0.0, pa, [&] { ring_prefetch(A.tm, W, R2); }, NoDeliver{});
+    // P2's home stream lands while this warp takes queue items and during the grid barrier; the logNorm P2 uses is
+    // computed by the block's first warp to get here (consumed after the next barrier)
+    run_phase<1, VBEM, true>(A, W, R1, bid, nblk, 0.0, 0.0, pa, [&] {
+      ring_prefetch(A.tm, W, R2);
+      if (VBEM && it > 0) lag_lognorm_first_warp(A, par, nblk, scratch);
+    }, NoDeliver{});
     SB_ACC_END(t1, 0)
     SB_DBG(1)
     grid.sync();
     SB_DBG(2)
     if (bid == 0 && threadIdx.x == 0) A.lq[0] = 0u;   // P1's work queue: idle until the next iteration
     if (VBEM && it > 0) logNorm = scratch[33];   // written before the grid barrier above
+    if (threadIdx.x == 0) *reinterpret_cast<unsigned int*>(&scratch[34]) = 0u;   // the next iteration's claim
     const double bias = (it == 0) ? A.first_bias : 0.0;  // alphasPrime starts at 1.0 (:812,:821)
     SB_DBG(3)
     SB_ACC_BEGIN(t2, 4)
@@ -989,7 +1000,7 @@ __global__ void __launch_bounds__(EM_THREADS, EM_MIN_BLOCKS) k_em_p2(const __gri
     if (it == 0) {
       logNorm = digamma_pos(A.sum0);
     } else {
-      lag_lognorm_warp0(A, par, gridDim.x, scratch);
+      if (threadIdx.x < 32) lag_lognorm_warp(A, par, gridDim.x, scratch);
       __syncthreads();
       logNorm = scratch[33];
     }

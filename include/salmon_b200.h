@@ -61,7 +61,8 @@ typedef struct sb_em_params {
   int32_t no_rich_eq;           /* sopt.noRichEqClasses */
   int32_t no_length_correction; /* sopt.noLengthCorrection */
   int32_t alt_init;             /* sopt.meta || sopt.alternativeInitMode */
-  int32_t reserved;
+  int32_t bootstrap_reproject;  /* sopt.bootstrapReproject: sb_bootstrap ends each replicate with one update against the
+                                   original class counts (CollapsedEMOptimizer.cpp:495-505); 0 = off */
   double vb_prior;              /* sopt.vbPrior (1e-2) */
   double tol;                   /* relDiffTolerance (0.01) */
   double num_required_frags;    /* sopt.numRequiredFragments (5e7) */
@@ -118,6 +119,14 @@ int sb_em_download(sb_em_ctx* ctx, double* alpha_out, sb_em_stats* stats);
 /* Debug/parity taps (tests): combinedWeights (:862-870) and validity flags. */
 int sb_em_get_combined(sb_em_ctx* ctx, double* combined_out, uint8_t* valid_out);
 
+/* The combined weights `--skipQuant --dumpEqWeights` writes (MappingPipelineStages.cpp:112-162): per class,
+ * count * w / max(eff_len, 1) normalised to sum 1 (w = 1 with no_rich_eq), computed on the device with the arithmetic
+ * of sb_em_prepare's combinedWeights.  eff_len = sb_map_result.eff_len (the transcript lengths under
+ * --noEffectiveLengthCorrection).  combined_out[eq->off[n_classes]].  Uploads the table into ctx (a later
+ * sb_em_prepare needs its own sb_em_upload). */
+int sb_eq_combined_weights(sb_em_ctx* ctx, const sb_eq_csr* eq, const double* eff_len, int no_rich_eq,
+                           double* combined_out);
+
 /* ---- bootstraps and Gibbs samples ----------------------------------------
  * Both run on the context sb_em_optimize (or upload+prepare+run) left behind: the class table,
  * combinedWeights, validity flags and effective lengths stay resident in HBM.  Each sample
@@ -131,7 +140,10 @@ typedef int (*sb_sample_cb)(const double* alpha, uint32_t n_txps, void* user);
  * src/inference/CollapsedEMOptimizer.cpp:554-690, doBootstrap :398-552).  p carries
  * min_iter = 50 (:411), tol, max_iter and the VBEM switch; num_mapped_frags is
  * readExp.numMappedFragments() (:572-573, used by the degenerate marking :608-621).
- * Returns 1 where doBootstrap returns false (:521-525). */
+ * Returns 1 where doBootstrap returns false (:521-525).  With p->bootstrap_reproject each replicate's converged
+ * alpha takes one more EM / VBEM update against the original counts of the classes the replicates resample, before
+ * the truncation (:495-505); that update drops a class whose denominator is at most DBL_MIN times the largest count of a
+ * multi-transcript class, so that count / denominator stays finite. */
 int sb_bootstrap(sb_em_ctx* ctx, const sb_em_params* p, double num_mapped_frags,
                  uint32_t n_bootstraps, uint64_t seed, sb_sample_cb cb, void* user);
 /* Parity tap: per input class, the count drawn by the last replicate.  Single-transcript classes
@@ -515,6 +527,8 @@ typedef struct sb_quant_opts {
   int32_t write_qualities;        /* --writeQualities: QUAL from the read files instead of '*' */
   int32_t write_unmapped_names;   /* --writeUnmappedNames: out_dir/aux_info/unmapped_names.txt */
   const char* cmdline;            /* the @PG CL: field of the SAM header (may be NULL) */
+  int32_t skip_quant;             /* --skipQuant: map and write the run metadata (and the classes with --dumpEq); no
+                                     normalizeAlphas, optimiser, quant.sf or samples (MappingPipelineStages.cpp:45-162) */
 } sb_quant_opts;
 typedef struct sb_quant_summary {
   uint64_t n_observed, n_mapped, n_too_short, n_trimmed_mates, n_classes, n_batches;
@@ -564,7 +578,9 @@ int sb_quant_eqclasses(const char* eq_path, const sb_em_params* ep, const sb_qua
  * "fast_dp" (ungapped shortcut of the DP kernel on/off), "chunk" (reads per pipeline chunk), "input_on_device"
  * (sb_map_batch's read pointers are device pointers: inputs already resident in HBM), "ascii_reads" (the read bytes
  * are sequence characters A/C/G/T/N as the reference's parser delivers them, klibpp::KSeq::seq, instead of base
- * codes).  Results are identical for every setting. */
+ * codes).  Results are identical for every setting.  "no_projection" = 1: sb_map_finish and
+ * sb_map_project_global skip normalizeAlphas' cluster projection and report projected_counts of 0 (a --skipQuant run,
+ * which has no optimiser to start); everything else they report is unchanged. */
 int sb_map_set_option(sb_map_ctx* ctx, const char* key, int64_t value);
 
 /* "lib_type" is also a key of sb_map_set_option: the expected library format of the batches that follow (inside the

@@ -41,7 +41,7 @@ class sb_em_params(C.Structure):
         ("no_rich_eq", C.c_int32),
         ("no_length_correction", C.c_int32),
         ("alt_init", C.c_int32),
-        ("reserved", C.c_int32),
+        ("bootstrap_reproject", C.c_int32),
         ("vb_prior", C.c_double),
         ("tol", C.c_double),
         ("num_required_frags", C.c_double),
@@ -145,7 +145,7 @@ class sb_quant_opts(C.Structure):
                 ("num_gibbs", C.c_uint32), ("thinning", C.c_uint32), ("no_gamma_draw", C.c_int32),
                 ("shard_index", C.c_uint32), ("shard_count", C.c_uint32), ("seed", C.c_uint64), ("nccl_uid", C.c_void_p),
                 ("write_mappings", C.c_char_p), ("write_qualities", C.c_int32), ("write_unmapped_names", C.c_int32),
-                ("cmdline", C.c_char_p)]
+                ("cmdline", C.c_char_p), ("skip_quant", C.c_int32)]
 
 
 class sb_read_meta(C.Structure):
@@ -202,6 +202,7 @@ SYMBOLS = {
     "sb_em_run": (C.c_int, [_P, C.POINTER(sb_em_stats)]),
     "sb_em_download": (C.c_int, [_P, _P, C.POINTER(sb_em_stats)]),
     "sb_em_get_combined": (C.c_int, [_P, _P, _P]),
+    "sb_eq_combined_weights": (C.c_int, [_P, _P, _P, C.c_int, _P]),
     "sb_em_set_option": (C.c_int, [_P, C.c_char_p, C.c_int64]),
     "sb_em_get_info": (C.c_int, [_P, C.c_char_p, C.POINTER(C.c_int64)]),
     "sb_em_debug_timeline": (C.c_int, [_P, _P, C.c_uint32]),
@@ -469,6 +470,18 @@ class EMContext:
         valid = np.empty(self._C, dtype=np.uint8)
         _check(self.lib.sb_em_get_combined(self.h, cw.ctypes.data, valid.ctypes.data), "sb_em_get_combined")
         return cw, valid
+
+    def combined_weights(self, eq: EqClasses, eff_len, no_rich_eq=False):
+        """sb_eq_combined_weights: the combined weights `--skipQuant --dumpEqWeights` writes, per class
+        count * w / max(eff_len, 1) normalised (w = 1 with no_rich_eq).  Replaces the table this context holds."""
+        eff_len = np.ascontiguousarray(eff_len, dtype=np.float64)
+        assert eff_len.shape[0] == eq.n_txps
+        out = np.empty(max(eq.nnz, 1), dtype=np.float64)
+        s = eq.as_struct()
+        _check(self.lib.sb_eq_combined_weights(self.h, C.byref(s), eff_len.ctypes.data, 1 if no_rich_eq else 0,
+                                               out.ctypes.data), "sb_eq_combined_weights")
+        self.M = 0
+        return out[:eq.nnz]
 
     def _collector(self):
         samples = []

@@ -79,11 +79,13 @@ int usage() {
           "                  [--mimicBT2 | --mimicStrictBT2] [--minAlnProb 1e-5]\n"
           "                  [--noFragLengthDist --noEffectiveLengthCorrection | --noEffectiveLengthCorrection]\n"
           "                  [--numBootstraps N | --numGibbsSamples N] [--thinningFactor 16] [--noGammaDraw] [--useEM] [--vbPrior 0.01]\n"
+          "                  [--bootstrapReproject] [--meta] [--alternativeInitMode] [--skipQuant]\n"
           "                  [--perNucleotidePrior] [--maxReadOcc 200] [--maxOccsPerHit 1000] [--minScoreFraction 0.65] [--consensusSlack 0.35]\n"
           "                  [--preMergeChainSubThresh 0.75] [--postMergeChainSubThresh 0.9] [--orphanChainSubThresh 0.95] [--allowDovetail]\n"
           "                  [--discardOrphansQuasi] [--hardFilter] [--rangeFactorizationBins 4] [--fldMean 250] [--fldSD 25] [--fldMax 1000] [--scoreExp 1]\n"
           "                  [--numPreAuxModelSamples 5000] [--numAuxModelSamples 5000000] [--gpu 0] [--batch 262144] [--maxReadLen 256] [--seed 42]\n"
-          "  sb_salmon quant -e eq_classes.txt[.gz] -o out_dir [--useEM] [--numBootstraps N]\n",
+          "  sb_salmon quant -e eq_classes.txt[.gz] -o out_dir [--useEM] [--numBootstraps N] [--bootstrapReproject] [--meta]\n"
+          "                  [--alternativeInitMode]\n",
           sb_version());
   return 1;
 }
@@ -215,6 +217,7 @@ int cmd_quant(Args& a) {
   auto num = [&](double& d) { if (!a.value(v)) return false; d = atof(v.c_str()); return true; };
   double d = 0;
   bool vb_prior_given = false, pre_merge_given = false, threads_given = false, mimic = false, mimic_strict = false;
+  bool meta = false;
   int n_gpus = 1, my_rank = -1;
   std::string run_tag, sam_path;
   while (a.more()) {
@@ -241,6 +244,10 @@ int cmd_quant(Args& a) {
     else if (o == "--initUniform") ep.init_uniform = 1;
     else if (o == "--noLengthCorrection") ep.no_length_correction = 1;
     else if (o == "--noRichEqClasses") ep.no_rich_eq = 1;
+    else if (o == "--meta") meta = true;
+    else if (o == "--alternativeInitMode") ep.alt_init = 1;
+    else if (o == "--bootstrapReproject") ep.bootstrap_reproject = 1;
+    else if (o == "--skipQuant") qo.skip_quant = 1;
     else if (o == "--maxReadOcc") { if (!num(d)) return usage(); mp.max_read_occ = (uint32_t)d; }
     else if (o == "--maxOccsPerHit") { if (!num(d)) return usage(); mp.max_occs_per_hit = (uint32_t)d; }
     else if (o == "--minScoreFraction") { if (!num(mp.min_score_fraction)) return usage(); }
@@ -312,6 +319,19 @@ int cmd_quant(Args& a) {
     } else { fprintf(stderr, "sb_salmon quant: unknown option %s\n", o.c_str()); return usage(); }
   }
   if (out.empty()) return usage();
+  if (meta) {   // a preset over the options given, whatever their order (QuantOptionsUtils.cpp:449-454)
+    ep.init_uniform = 1;
+    ep.no_rich_eq = 1;
+    ep.use_vbem = 0;
+    ep.alt_init = 1;   // (metaGenomeMode, CollapsedEMOptimizer.cpp:800-810; no effect beside initUniform)
+    if (my_rank <= 0)
+      fprintf(stderr, "[info] --meta sets --useEM --initUniform --noRichEqClasses, whatever else the command line says "
+                      "about them.\n");
+  }
+  if (qo.skip_quant && !eqfile.empty()) {
+    fprintf(stderr, "sb_salmon quant: --skipQuant applies to mapping mode; with --eqclasses there is nothing to skip to\n");
+    return 1;
+  }
   if (mimic && mimic_strict) {   // QuantOptionsUtils.cpp:250-254
     fprintf(stderr, "sb_salmon quant: You passed both the --mimicBT2 and --mimicStrictBT2 parameters.  These are mutually "
                     "exclusive. Please select only one of these flags.\n");

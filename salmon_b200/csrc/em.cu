@@ -74,6 +74,24 @@ __global__ void k_txp_init(uint32_t M, const double* __restrict__ projected,
   alpha0[i] = a;
 }
 
+// :830-873 (and MappingPipelineStages.cpp:116-125): the combined weight of every entry of one class before the
+// normalisation, written to cw[b, e); returns their sum
+__device__ __forceinline__ double class_weights(uint64_t b, uint64_t e, double count, const uint32_t* __restrict__ tids,
+                                                const double* __restrict__ aux, const double* __restrict__ effLens,
+                                                int no_rich_eq, int eq_class_mode, double* __restrict__ cw) {
+  double wsum = 0.0;
+  for (uint64_t j = b; j < e; ++j) {
+    double el = effLens[tids[j]];
+    if (el <= 1.0) el = 1.0;
+    double w = no_rich_eq ? 1.0 : aux[j];
+    double probStartPos = 1.0 / el;
+    double wt = eq_class_mode ? w : __dmul_rn(__dmul_rn(count, w), probStartPos);
+    cw[j] = wt;
+    wsum = __dadd_rn(wsum, wt);
+  }
+  return wsum;
+}
+
 // :830-873 combined weights, :330-394 degenerate marking, singleton folding.
 // One thread per class (one-time work).  sortkey = first transcript of a kept class.
 __global__ void k_class_combine(uint64_t C, uint32_t M, const uint64_t* __restrict__ off,
@@ -90,16 +108,7 @@ __global__ void k_class_combine(uint64_t C, uint32_t M, const uint64_t* __restri
   if (c >= C) return;
   const uint64_t b = off[c], e = off[c + 1];
   const double count = (double)counts[c];
-  double wsum = 0.0;
-  for (uint64_t j = b; j < e; ++j) {
-    double el = effLens[tids[j]];
-    if (el <= 1.0) el = 1.0;
-    double w = p.no_rich_eq ? 1.0 : aux[j];
-    double probStartPos = 1.0 / el;
-    double wt = p.eq_class_mode ? w : __dmul_rn(__dmul_rn(count, w), probStartPos);
-    cw[j] = wt;
-    wsum = __dadd_rn(wsum, wt);
-  }
+  const double wsum = class_weights(b, e, count, tids, aux, effLens, p.no_rich_eq, p.eq_class_mode, cw);
   const double wnorm = 1.0 / wsum;
   double denom = 0.0;
   for (uint64_t j = b; j < e; ++j) {
@@ -126,6 +135,17 @@ __global__ void k_class_combine(uint64_t C, uint32_t M, const uint64_t* __restri
   packed[c] = pk;
   sortkey[c] = key;
   cls_map[c] = cmap;
+}
+
+// --skipQuant --dumpEqWeights (MappingPipelineStages.cpp:112-162): the combined weights alone, normalised per class
+__global__ void k_eq_combined(uint64_t C, const uint64_t* __restrict__ off, const uint32_t* __restrict__ tids,
+                              const double* __restrict__ aux, const uint64_t* __restrict__ counts,
+                              const double* __restrict__ effLens, int no_rich_eq, double* __restrict__ cw) {
+  uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const uint64_t b = off[c], e = off[c + 1];
+  const double wnorm = 1.0 / class_weights(b, e, (double)counts[c], tids, aux, effLens, no_rich_eq, 0, cw);
+  for (uint64_t j = b; j < e; ++j) cw[j] = __dmul_rn(cw[j], wnorm);
 }
 
 // second-level key: (locality group, length bucket); dropped rows last
@@ -1482,6 +1502,49 @@ extern "C" int sb_em_get_combined(sb_em_ctx* c, double* combined_out, uint8_t* v
   if (combined_out && c->nnz)
     SB_CUDA(cudaMemcpy(combined_out, c->d_cw, c->nnz * 8, cudaMemcpyDeviceToHost));
   if (valid_out && c->C) SB_CUDA(cudaMemcpy(valid_out, c->d_valid, c->C, cudaMemcpyDeviceToHost));
+  return SB_OK;
+}
+
+extern "C" int sb_eq_combined_weights(sb_em_ctx* c, const sb_eq_csr* eq, const double* eff_len, int no_rich_eq,
+                                      double* combined_out) {
+  if (!c || !eq || !eff_len || !combined_out) { set_error("null argument"); return SB_ERR_INVALID; }
+  const uint32_t M = eq->n_txps;
+  std::vector<double> zeros(M, 0.0);   // the projected and unique counts play no part here
+  std::vector<uint64_t> uzeros(M, 0);
+  SB_TRY(sb_em_upload(c, eq, zeros.data(), eff_len, uzeros.data()));
+  const uint64_t C = c->C, nnz = c->nnz;
+  if (!nnz) return SB_OK;
+  cudaStream_t st = c->stream;
+  SB_TRY(c->res.grow(&c->d_cw, nnz));
+  k_eq_combined<<<nblk(C, 128), 128, 0, st>>>(C, c->d_off, c->d_tids, c->d_aux, c->d_counts, c->d_eff_in,
+                                               no_rich_eq ? 1 : 0, c->d_cw);
+  SB_CUDA(cudaGetLastError());
+  SB_CUDA(cudaMemcpyAsync(combined_out, c->d_cw, nnz * 8, cudaMemcpyDeviceToHost, st));
+  SB_CUDA(cudaStreamSynchronize(st));
+  return SB_OK;
+}
+
+// --bootstrapReproject (CollapsedEMOptimizer.cpp:495-505): one more update of the single-GPU loop, from the alpha and
+// theta the last sb_em_run left in row space, against the class counts `cnt` (compact classes) and the folded
+// singleton counts base_row / base_tid, dropping classes whose denominator is at most min_eq_w.  The iteration index
+// continues the run's, so P2's lagged logNorm reads the partial sums the run's last iteration wrote.  The result
+// replaces d_alpha.
+static int em_reproject(sb_em_ctx* c, const double* cnt, const double* base_row, const double* base_tid,
+                        double min_eq_w) {
+  cudaStream_t st = c->stream;
+  const int vb = c->params.use_vbem ? 1 : 0;
+  const uint32_t it = c->iters;
+  EmArgs A;
+  fill_args(c, A, true);
+  A.c_cnt = cnt;
+  A.base = base_row;
+  A.min_eq_w = min_eq_w;
+  k_reset_maxrel<<<1, 1, 0, st>>>(A.maxrel, it & 1u);
+  K_P1[vb]<<<c->grid, EM_THREADS, EM_SMEM, st>>>(A);
+  K_P2[vb]<<<c->grid, EM_THREADS, EM_SMEM, st>>>(A, it);
+  k_finalize<<<nblk(c->M, 256), 256, 0, st>>>(c->M, c->d_tid_row, base_tid, 0.0, c->r_alpha, c->d_alpha);
+  SB_CUDA(cudaGetLastError());
+  c->launches += 4;
   return SB_OK;
 }
 

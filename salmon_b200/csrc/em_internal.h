@@ -135,6 +135,10 @@ struct sb_em_ctx {
   double* ov_alpha0_row = nullptr;
   double* ov_alpha0_tid = nullptr;
   double ov_sum0 = 0.0, ov_inactive_sum = 0.0, ov_min_eq_w = 0.0;
+  // --bootstrapReproject: the original counts of the classes the replicates resample, in the overlay's layout
+  double* rp_cnt = nullptr;
+  double* rp_base_row = nullptr;
+  double* rp_base_tid = nullptr;
   // sampling scratch
   uint64_t* d_cdf = nullptr;
   uint32_t* d_cls_map = nullptr;

@@ -984,6 +984,7 @@ struct sb_map_ctx {
   int input_dev = 0;                 // sb_map_batch's read pointers are device pointers (bench: inputs resident in HBM)
   int ascii = 0;                     // reads are sequence characters (ACGTN...) instead of base codes
   int fast_ok = 1;
+  int no_projection = 0;             // finish without normalizeAlphas' cluster projection (--skipQuant)
   uint32_t k1_threads = 0, seed_blocks = 0, dp_blocks = 0;
   BatchBufs b{};                     // cand/score/task buffers: one chunk; outputs: whole batch
   // k_assign of chunk i runs on its own stream next to the seed / DP kernels of chunk i+1 (it is latency-bound at
@@ -1365,6 +1366,7 @@ extern "C" int sb_map_set_option(sb_map_ctx* c, const char* key, int64_t value) 
     c->d_dummy_mate = nullptr;
     return SB_OK;
   }
+  if (!strcmp(key, "no_projection")) { c->no_projection = value ? 1 : 0; return SB_OK; }
   if (!strcmp(key, "overlap_assign")) { c->overlap_assign = value ? 1 : 0; return SB_OK; }
   if (!strcmp(key, "sam_window_bytes")) {
     if (value < 1) { sb::set_error("sam_window_bytes must be positive"); return SB_ERR_INVALID; }
@@ -1861,23 +1863,26 @@ static int finish_project(sb_map_ctx* c) {
   c->h_proj.assign(M, 0.0); c->h_eff.assign(M, 0.0); c->h_uniq.assign(M, 0); c->h_total.assign(M, 0);
   if (!M) return SB_OK;
   FinBufs& f = c->fin;
-  size_t t2 = f.tmp_bytes;
-  SB_CUDA(cub::DeviceRadixSort::SortPairs(f.tmp, t2, f.root, f.root2, f.ids, f.memb, (int)M, 0, 32, st));   // stable: members ascending
-  k_cluster_heads<<<nblk((uint64_t)M + 1, 256), 256, 0, st>>>(M, f.root2, f.head);
-  t2 = f.tmp_bytes;
-  SB_CUDA(cub::DeviceScan::ExclusiveSum(f.tmp, t2, f.head, f.head_scan, (int)M + 1, st));
-  uint32_t ncl = 0;
-  SB_CUDA(cudaMemcpyAsync(&ncl, f.head_scan + M, 4, cudaMemcpyDeviceToHost, st));
-  SB_CUDA(cudaStreamSynchronize(st));
-  k_cluster_starts<<<nblk(M, 256), 256, 0, st>>>(M, f.head, f.head_scan, f.start);
-  k_cluster_project<<<nblk((uint64_t)ncl * 32, 256), 256, 0, st>>>(ncl, M, f.start, f.memb, c->on.mass, f.hits, f.uniq,
-                                                                   f.total, f.proj, f.bound);
+  if (!c->no_projection) {
+    size_t t2 = f.tmp_bytes;
+    SB_CUDA(cub::DeviceRadixSort::SortPairs(f.tmp, t2, f.root, f.root2, f.ids, f.memb, (int)M, 0, 32, st));   // stable: members ascending
+    k_cluster_heads<<<nblk((uint64_t)M + 1, 256), 256, 0, st>>>(M, f.root2, f.head);
+    t2 = f.tmp_bytes;
+    SB_CUDA(cub::DeviceScan::ExclusiveSum(f.tmp, t2, f.head, f.head_scan, (int)M + 1, st));
+    uint32_t ncl = 0;
+    SB_CUDA(cudaMemcpyAsync(&ncl, f.head_scan + M, 4, cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaStreamSynchronize(st));
+    k_cluster_starts<<<nblk(M, 256), 256, 0, st>>>(M, f.head, f.head_scan, f.start);
+    k_cluster_project<<<nblk((uint64_t)ncl * 32, 256), 256, 0, st>>>(ncl, M, f.start, f.memb, c->on.mass, f.hits, f.uniq,
+                                                                     f.total, f.proj, f.bound);
+    c->launches += 6;
+  }
   if (c->p.no_eff_len_correction)   // --noEffectiveLengthCorrection: transcript lengths (CollapsedEMOptimizer.cpp:611-613,786-788)
     k_tx_len<<<nblk(M, 256), 256, 0, st>>>(M, c->index->d_tx_off, f.eff);
   else
     k_exp_vec<<<nblk(M, 256), 256, 0, st>>>(M, c->on.log_eff, f.eff);     // CollapsedEMOptimizer.cpp:782-784
-  c->launches += 7;
-  SB_CUDA(cudaMemcpyAsync(c->h_proj.data(), f.proj, (size_t)M * 8, cudaMemcpyDeviceToHost, st));
+  c->launches += 1;
+  if (!c->no_projection) SB_CUDA(cudaMemcpyAsync(c->h_proj.data(), f.proj, (size_t)M * 8, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaMemcpyAsync(c->h_eff.data(), f.eff, (size_t)M * 8, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaMemcpyAsync(c->h_uniq.data(), f.uniq, (size_t)M * 8, cudaMemcpyDeviceToHost, st));
   SB_CUDA(cudaMemcpyAsync(c->h_total.data(), f.total, (size_t)M * 8, cudaMemcpyDeviceToHost, st));

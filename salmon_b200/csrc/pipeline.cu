@@ -713,6 +713,8 @@ extern "C" int sb_quant_files(sb_index* ix, const char* const* mates1, const cha
   }
 
   // ---- classes -> (global statistics) -> EM -> outputs -----------------------------------------------------------
+  // --skipQuant: no normalizeAlphas (MappingPipelineStages.cpp:45-47), so finish without the cluster projection
+  if (o.skip_quant) SB_TRY(sb_map_set_option(S.ctx, "no_projection", 1));
   sb_map_result res;
   rc = sb_map_finish(S.ctx, &res);
   if (rc != SB_OK) return rc;
@@ -724,14 +726,23 @@ extern "C" int sb_quant_files(sb_index* ix, const char* const* mates1, const cha
   std::vector<double> alpha(M, 0.0);
   sb_em_stats est;
   memset(&est, 0, sizeof est);
-  S.em = sb_em_create(o.device);
-  if (!S.em) return SB_ERR_CUDA;
-  if (multi) SB_TRY(sb_em_peer_setup(S.em, S.comm, Mq));
-  rc = sb_em_optimize(S.em, &eq, &ep, glob.projected_counts, glob.eff_len, glob.unique_counts, alpha.data(), &est);
+  // --skipQuant --dumpEqWeights: the dumped weights are the combined weights (MappingPipelineStages.cpp:112-162)
+  std::vector<double> combined;
+  if (!o.skip_quant || o.dump_eq_weights) {
+    S.em = sb_em_create(o.device);
+    if (!S.em) return SB_ERR_CUDA;
+  }
+  if (!o.skip_quant) {
+    if (multi) SB_TRY(sb_em_peer_setup(S.em, S.comm, Mq));
+    rc = sb_em_optimize(S.em, &eq, &ep, glob.projected_counts, glob.eff_len, glob.unique_counts, alpha.data(), &est);
+    if (rc < 0) return rc;
+    if (rc == 1) { sb::set_error("The optimization algorithm failed (total alpha weight too small)"); return SB_ERR_STATE; }
+  } else if (o.dump_eq_weights && out_dir && o.shard_index == 0) {
+    combined.resize((res.n_classes ? res.off[res.n_classes] : 0) + 1);   // (+1: a table with no entries still has weights)
+    SB_TRY(sb_eq_combined_weights(S.em, &eq, glob.eff_len, ep.no_rich_eq, combined.data()));
+  }
   const double n_mapped = (double)n_mapped_u;
   std::string outs = out_dir ? out_dir : "";
-  if (rc < 0) return rc;
-  if (rc == 1) { sb::set_error("The optimization algorithm failed (total alpha weight too small)"); return SB_ERR_STATE; }
   const double t_em = now_s();
   std::vector<std::string> gen;
   std::vector<const char*> np;
@@ -753,10 +764,12 @@ extern "C" int sb_quant_files(sb_index* ix, const char* const* mates1, const cha
       for (uint32_t t = 0; t < M; ++t) lens.push_back((uint32_t)(off[t + 1] - off[t]));
       complete_len = lens.data();
     }
-    rc = sb_write_quant_sf((outs + "/quant.sf").c_str(), Mq, names, complete_len, glob.eff_len, alpha.data(), n_mapped, 3);
+    rc = o.skip_quant ? SB_OK
+                      : sb_write_quant_sf((outs + "/quant.sf").c_str(), Mq, names, complete_len, glob.eff_len, alpha.data(),
+                                          n_mapped, 3);
     if (rc == SB_OK && (o.dump_eq || o.dump_eq_weights))
       rc = sb_write_eq_classes((outs + "/aux_info/eq_classes.txt.gz").c_str(), Mq, names, res.n_classes, res.off, res.tids,
-                               o.dump_eq_weights ? res.weights : nullptr, res.counts);
+                               o.dump_eq_weights ? (o.skip_quant ? combined.data() : res.weights) : nullptr, res.counts);
     if (rc != SB_OK) return rc;
     // run metadata
     std::vector<double> hist((size_t)mp.max_frag_len + 1, 0.0);
@@ -770,7 +783,7 @@ extern "C" int sb_quant_files(sb_index* ix, const char* const* mates1, const cha
               glob.n_compatible};
     SB_TRY(write_run_metadata(outs, mi));
   }
-  if (o.num_bootstraps || o.num_gibbs) {
+  if ((o.num_bootstraps || o.num_gibbs) && !o.skip_quant) {   // --skipQuant draws no samples (its help text)
     rc = run_samples(S.em, ep, o, alpha.data(), Mq, n_mapped, nullptr, o.shard_index == 0 ? outs : std::string(), names);
     if (rc < 0) return rc;
   }

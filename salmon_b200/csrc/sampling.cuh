@@ -100,6 +100,23 @@ __global__ void k_boot_sample(uint64_t total, uint32_t b, uint32_t k0, uint32_t 
     else atomicAdd(&samp_multi[m], 1ull);
   }
 }
+// --bootstrapReproject: the original count of every class a replicate resamples, into the accumulators the draws go to;
+// max_multi = the largest count of a multi-transcript class (the reprojection's denominator guard)
+__global__ void k_boot_orig_counts(uint64_t C, const uint64_t* __restrict__ counts,
+                                   const uint8_t* __restrict__ valid_boot, const uint32_t* __restrict__ cls_map,
+                                   unsigned long long* __restrict__ samp_multi,
+                                   unsigned long long* __restrict__ samp_single, unsigned long long* __restrict__ max_multi) {
+  uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C || !valid_boot[c]) return;
+  const uint32_t m = cls_map[c];
+  if (m == 0xffffffffu) return;
+  if (m & 0x80000000u) {
+    atomicAdd(&samp_single[m & 0x7fffffffu], (unsigned long long)counts[c]);   // integer: order free
+  } else {
+    atomicAdd(&samp_multi[m], (unsigned long long)counts[c]);
+    atomicMax(max_multi, (unsigned long long)counts[c]);
+  }
+}
 __global__ void k_u64_to_f64(uint64_t n, const unsigned long long* __restrict__ a, double* __restrict__ o) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) o[i] = (double)a[i];
@@ -302,6 +319,33 @@ extern "C" int sb_bootstrap(sb_em_ctx* c, const sb_em_params* p, double num_mapp
   SB_TRY(build_cdf(c, c->d_valid_boot, 0, &total));
   if (total == 0) { set_error("no fragments to resample"); return SB_ERR_INVALID; }
   const double unif = scale * (double)total;                                         // :450-453, :681
+  // --bootstrapReproject (:495-505): the update after each replicate's loop runs over the same classes (txpGroups, the
+  // valid_boot ones) with their original counts (origCounts).  d_counts is the uploaded table, which the resampling only
+  // reads: the counts are laid out once, as the draws are, and stay resident for every replicate.
+  // The update drops a class whose denominator is at most DBL_MIN times the largest multi-transcript count, the
+  // degenerate-class rule (denom <= minEQClassWeight, :143-145) scaled so that count / denom stays finite.  A class the
+  // replicate did not draw has members it drove to zero or to subnormal values; with salmon's guards the quotient
+  // overflows and the replicate would carry infinities (or 0 * inf = NaN).
+  const bool reproject = p->bootstrap_reproject != 0 && n_boot > 0;
+  double rp_min_eq_w = DBL_MIN;
+  if (reproject) {
+    SB_TRY(c->res.grow(&c->rp_cnt, (size_t)Cm + 1));
+    SB_TRY(c->res.grow(&c->rp_base_tid, (size_t)M));
+    SB_TRY(c->res.grow(&c->rp_base_row, (size_t)R + 1));
+    SB_CUDA(cudaMemsetAsync(c->d_samp, 0, ((size_t)Cm + M + 1) * 8, st));
+    unsigned long long* d_max = (unsigned long long*)(c->d_scalars + 42);
+    SB_CUDA(cudaMemsetAsync(d_max, 0, 8, st));
+    if (C) k_boot_orig_counts<<<nblk(C, 256), 256, 0, st>>>(C, c->d_counts, c->d_valid_boot, c->d_cls_map, c->d_samp,
+                                                             c->d_samp + Cm, d_max);
+    if (Cm) k_u64_to_f64<<<nblk(Cm, 256), 256, 0, st>>>(Cm, c->d_samp, c->rp_cnt);
+    k_u64_to_f64<<<nblk(M, 256), 256, 0, st>>>(M, c->d_samp + Cm, c->rp_base_tid);
+    if (R) k_boot_rows<<<nblk(R, 256), 256, 0, st>>>(R, c->d_row_tid, c->rp_base_tid, unif, c->rp_base_row,
+                                                      c->ov_alpha0_row);
+    unsigned long long max_multi = 0;
+    SB_CUDA(cudaMemcpyAsync(&max_multi, d_max, 8, cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaStreamSynchronize(st));
+    rp_min_eq_w = DBL_MIN * (double)std::max(1ull, max_multi);
+  }
   // restores the context on EVERY exit path (the SB_CUDA macros below return early on a CUDA error)
   struct Restore {
     sb_em_ctx* c; sb_em_params saved;
@@ -331,6 +375,7 @@ extern "C" int sb_bootstrap(sb_em_ctx* c, const sb_em_params* p, double num_mapp
     c->ov_min_eq_w = p->use_vbem ? DBL_MIN : 4.9406564584124654e-324;   // :153 vs EMUtils.cpp:36
     sb_em_stats stt;
     int rc = sb_em_run(c, &stt);
+    if (rc == SB_OK && reproject) rc = em_reproject(c, c->rp_cnt, c->rp_base_row, c->rp_base_tid, rp_min_eq_w);
     c->ov_active = false;
     if (rc != SB_OK) { rc_out = rc; break; }
     rc = sb_em_download(c, alpha.data(), &stt);

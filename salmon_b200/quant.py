@@ -27,6 +27,22 @@ def _boot_params(ep):
     return bp
 
 
+def _em_options(ep, meta=False, alternative_init_mode=False, bootstrap_reproject=False):
+    """salmon's offline-phase options on em_params (DESIGN.md section 15): `--alternativeInitMode`,
+    `--bootstrapReproject`, then the `--meta` preset, which overrides the values given for the same options
+    (QuantOptionsUtils.cpp:449-454); the defaults leave ep as it is"""
+    if alternative_init_mode:
+        ep.alt_init = 1
+    if bootstrap_reproject:
+        ep.bootstrap_reproject = 1
+    if meta:
+        ep.init_uniform = 1
+        ep.no_rich_eq = 1
+        ep.use_vbem = 0
+        ep.alt_init = 1      # metaGenomeMode (CollapsedEMOptimizer.cpp:800-810): no effect beside initUniform
+    return ep
+
+
 def _likelihood_options(mp, incompat_prior, no_single_frag_prob, no_frag_len_dist, no_eff_len_correction):
     """salmon's fragment-likelihood options on map_params (DESIGN.md section 13); the defaults leave mp as it is"""
     if incompat_prior:
@@ -127,11 +143,13 @@ def quant_reads(index, left, right, map_params=None, em_params=None, device=0, b
 
 
 def _quantify(index, ctx, ep, device, dist, names, out_dir, dump_eq, dump_eq_weights, num_bootstraps=0, seed=0,
-              n_observed=None):
+              n_observed=None, skip_quant=False):
     """Everything after mapping: finish() -> (multi-GPU reduction) -> EM -> outputs.  Shared by quant_reads-style
     callers that drive the MapContext themselves."""
     world = dist.get_world_size() if (dist is not None and dist.is_initialized()) else 1
     rank = dist.get_rank() if world > 1 else 0
+    if skip_quant:
+        return _skip_quant(index, ctx, device, dist, names, out_dir, dump_eq, dump_eq_weights, ep, n_observed)
     res = ctx.finish()
     inputs = res
     n_mapped = res["counters"]["n_mapped"]
@@ -176,11 +194,46 @@ def _quantify(index, ctx, ep, device, dist, names, out_dir, dump_eq, dump_eq_wei
                 n_observed=n_observed)
 
 
+def _skip_quant(index, ctx, device, dist, names, out_dir, dump_eq, dump_eq_weights, ep, n_observed):
+    """`--skipQuant` (MappingPipelineStages.cpp:45-162): the classes without normalizeAlphas' projection, no optimiser,
+    no quant.sf, no samples; under dump_eq_weights the dumped weights are the combined weights, computed on the device
+    (sb_eq_combined_weights)"""
+    world = dist.get_world_size() if (dist is not None and dist.is_initialized()) else 1
+    rank = dist.get_rank() if world > 1 else 0
+    ctx.set_option("no_projection", 1)
+    res = ctx.finish()
+    inputs = res
+    n_mapped = res["counters"]["n_mapped"]
+    if world > 1:
+        from .dist import reduce_partials
+        g, roots = reduce_partials(ctx.partial(), dist, f"cuda:{device}")
+        inputs = ctx.project_global(g, roots)
+        n_mapped = g["assigned"]
+    ctx.close()
+    M, inputs = _drop_decoys(index, inputs)
+    combined = None
+    if dump_eq_weights:
+        em = EMContext(device)
+        combined = em.combined_weights(EqClasses(M, res["off"], res["tids"], res["weights"], res["counts"]),
+                                       inputs["eff_len"], no_rich_eq=bool(ep.no_rich_eq))
+        em.close()
+    if out_dir is not None and rank == 0 and (dump_eq or dump_eq_weights):
+        os.makedirs(os.path.join(out_dir, "aux_info"), exist_ok=True)
+        meta = index.meta()
+        nm = (names or meta["names"] or [f"t{i}" for i in range(index.n_txps)])[:M]
+        _capi.write_eq_classes(os.path.join(out_dir, "aux_info", "eq_classes.txt.gz"), nm, res["off"], res["tids"],
+                               res["counts"], combined)
+    return dict(alpha=None, tpm=None, eff_len=inputs["eff_len"], classes=res, n_mapped=int(n_mapped), em_stats=None,
+                projected_counts=None, unique_counts=inputs["unique_counts"], bootstraps=None, n_observed=n_observed,
+                combined_weights=combined)
+
+
 def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=None, device=0, batch=262_144,
                 max_read_len=256, threads=8, dist=None, dump_eq=False, dump_eq_weights=False, num_bootstraps=0, seed=0,
                 write_mappings=None, write_qualities=False, write_unmapped_names=False, cmdline="", recover_orphans=False,
                 softclip=0, incompat_prior=0.0, no_single_frag_prob=False, no_frag_len_dist=False,
-                no_eff_len_correction=False, min_aln_prob=None, mimic_bt2=False, mimic_strict_bt2=False):
+                no_eff_len_correction=False, min_aln_prob=None, mimic_bt2=False, mimic_strict_bt2=False,
+                skip_quant=False, bootstrap_reproject=False, meta=False, alternative_init_mode=False):
     """`salmon quant -i index -l IU -1 mates1 -2 mates2 -o out_dir` for the hot path: FASTQ/FASTA(.gz) files ->
     sb_reads_bucketed -> sb_map_batch -> ... -> quant.sf.  index: an _capi.Index or the path of a saved one.  With
     torch.distributed initialised every rank takes the global batches g with g % world == rank (round-robin sharding
@@ -193,7 +246,9 @@ def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=
     `--softclip` (DESIGN.md section 12).  incompat_prior, no_single_frag_prob, no_frag_len_dist, no_eff_len_correction:
     `--incompatPrior`, `--noSingleFragProb`, `--noFragLengthDist`, `--noEffectiveLengthCorrection` (DESIGN.md section
     13).  min_aln_prob, mimic_bt2, mimic_strict_bt2: `--minAlnProb`, `--mimicBT2`, `--mimicStrictBT2`, applied after the
-    other options so that the presets override them (DESIGN.md section 14)."""
+    other options so that the presets override them (DESIGN.md section 14).  skip_quant, bootstrap_reproject, meta,
+    alternative_init_mode: `--skipQuant`, `--bootstrapReproject`, `--meta`, `--alternativeInitMode` (DESIGN.md section
+    15); with skip_quant the result has no alpha and, under dump_eq_weights, the combined weights."""
     if isinstance(index, (str, bytes, os.PathLike)):
         index = _capi.Index.load(index)
     mp = map_params or map_default_params()
@@ -203,10 +258,10 @@ def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=
         mp.softclip = int(softclip)
     _likelihood_options(mp, incompat_prior, no_single_frag_prob, no_frag_len_dist, no_eff_len_correction)
     _mimic_options(mp, min_aln_prob, mimic_bt2, mimic_strict_bt2)
-    meta = index.meta()
-    if meta["first_decoy"] < index.n_txps:
-        mp.first_decoy = meta["first_decoy"]
-    ep = em_params or default_params()
+    first_decoy = index.meta()["first_decoy"]
+    if first_decoy < index.n_txps:
+        mp.first_decoy = first_decoy
+    ep = _em_options(em_params or default_params(), meta, alternative_init_mode, bootstrap_reproject)
     world = dist.get_world_size() if (dist is not None and dist.is_initialized()) else 1
     rank = dist.get_rank() if world > 1 else 0
     ctx = MapContext(index, mp, device=device, batch_cap=batch, max_read_len=max_read_len)
@@ -246,12 +301,14 @@ def quant_files(index, mates1, mates2, out_dir=None, map_params=None, em_params=
                              shard_index=rank, shard_count=world)
     n_observed = int(st["n_observed"])
     return _quantify(index, ctx, ep, device, dist, None, out_dir, dump_eq, dump_eq_weights, num_bootstraps, seed,
-                     n_observed=n_observed)
+                     n_observed=n_observed, skip_quant=skip_quant)
 
 
-def quant_eqclasses(eq_path, out_dir=None, em_params=None, device=0, num_bootstraps=0, seed=0):
+def quant_eqclasses(eq_path, out_dir=None, em_params=None, device=0, num_bootstraps=0, seed=0,
+                    bootstrap_reproject=False, meta=False, alternative_init_mode=False):
     """`salmon quant --eqclasses eq_classes.txt[.gz]` (EM only; src/quant/SalmonQuantify.cpp eq-class mode ->
-    CollapsedEMOptimizer::optimize with eq_class_mode): BASELINE.json configs[1]."""
+    CollapsedEMOptimizer::optimize with eq_class_mode): BASELINE.json configs[1].  bootstrap_reproject, meta,
+    alternative_init_mode: `--bootstrapReproject`, `--meta`, `--alternativeInitMode` (DESIGN.md section 15)."""
     f = _capi.read_eq_classes(eq_path)
     if not f["has_weights"]:
         raise _capi.SalmonB200Error("--eqclasses input needs the weights (write it with --dumpEqWeights)")
@@ -261,7 +318,7 @@ def quant_eqclasses(eq_path, out_dir=None, em_params=None, device=0, num_bootstr
     # no unique counts), initUniform + eqClassMode, effective lengths taken from the file as they are
     projected = np.zeros(M)
     uniq = np.zeros(M, dtype=np.uint64)
-    ep = em_params or default_params()
+    ep = _em_options(em_params or default_params(), meta, alternative_init_mode, bootstrap_reproject)
     ep.eq_class_mode = 1
     ep.init_uniform = 1
     em = EMContext(device)
